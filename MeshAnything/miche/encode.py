@@ -4,7 +4,7 @@ encoder object `MeshAnything` holds as `self.point_encoder`.
 The reference builds a Lightning-era module tree from `shapevae-256.yaml` with OmegaConf and runs it with
 PyTorch ops.  Here the module is a thin handle: its weights arrive through
 `MeshAnything.load_state_dict` (keys `point_encoder.model.shape_model.*`) and its two entry points
-call the sm_100a kernels through the C ABI (`ma_encoder_forward`).  The yaml values are constants of
+call the sm_90a kernels through the C ABI (`ma_encoder_forward`).  The yaml values are constants of
 `meshanything_b200.config.ENC`.
 """
 from __future__ import annotations

@@ -1,6 +1,6 @@
 """Drop-in for /root/reference/MeshAnything/models/meshanything.py: same import path, constructor,
 `load_state_dict(strict=True)` key set and `forward(pc_normal, sampling=False)` contract
-(SURVEY.md 8b), with every arithmetic stage running in libmeshanything_b200.so (sm_100a):
+(SURVEY.md 8b), with every arithmetic stage running in libmeshanything_b200.so (sm_90a):
 
     forward (meshanything.py:134-176)
       point_encoder.encode_latents + process_point_feature  -> ma_encoder_forward

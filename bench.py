@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- face-tokens/sec of the MeshAnything-350M hot path on B200 (BASELINE.json metric).
+"""bench.py -- face-tokens/sec of the MeshAnything-350M hot path on H100 (BASELINE.json metric).
 
 One "step" = one full pass of the hot path over one batch of synthetic inputs: generate()
 of `--faces`*9+2 tokens for `--batch` shapes per GPU (default: BASELINE.json configs[1] = batch 1,
@@ -41,11 +41,11 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "fallback (H100 SXM data sheet HBM3 bandwidth)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks + throttle reasons sampled DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -211,13 +211,31 @@ def batched_decode_steps(arena, n_layers, B, F, sampling, contexts, steps=200, w
     return {"batch_per_gpu": B, "faces": F, "sampling": bool(sampling), "kv_cache_GB": kv_bytes / 1e9,
             "steps_timed_per_context": steps, "contexts": rows, "tokens_per_s_over_contexts": tps,
             "peak_GBps": peak, "peak_source": peak_src,
-            "kernels": "gemm_ws_kernel (tcgen05, swap-AB, K slices in a cluster) + attention_stream_kernel + sample_kernel in one CUDA graph per step"
+            "kernels": "gemm_ws_kernel (wgmma, swap-AB, K slices in a cluster) + attention_stream_kernel + sample_kernel in one CUDA graph per step"
                        if sampling else "gemm_canon_kernel + attention_stream_kernel + sample_kernel in one CUDA graph per step",
             "note": "decode steps only (no encoder / prefill / detokenizer); KV zero-filled, state set by ma_decode_slots_seek"}
 
 
 CONFIGS = {2: dict(batch=1, faces=800, sampling=False), 3: dict(batch=64, faces=800, sampling=True),
            4: dict(batch=64, faces=800, sampling=True), 5: dict(batch=32, faces=1600, sampling=True)}
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Each array as out_dir/<name>.npy in float32; one larger than DUMP_LIMIT_BYTES is cut to a fixed, seeded sample
+    of its leading-dimension rows, so that two builds can be compared output for output."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    budget = DUMP_LIMIT_BYTES // max(1, len(arrays))
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        if a.nbytes > budget and a.ndim > 0:
+            keep = max(1, int(a.shape[0] * budget // a.nbytes))
+            rows = np.sort(np.random.default_rng(0).choice(a.shape[0], size=keep, replace=False))
+            a = a[rows]
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 def main():
@@ -237,6 +255,8 @@ def main():
     ap.add_argument("--sampling", action="store_true")
     ap.add_argument("--flags", type=int, default=0)
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step returned (the meshes of MeshAnything.forward) as DIR/<name>.npy")
     args = ap.parse_args()
     cfg = CONFIGS[args.config]
     if args.batch is None:
@@ -314,6 +334,9 @@ def main():
     tmax = 257 + max_new
     gen = model._generator(B)
     flags = args.flags | capi.GEN_NO_EARLY_EXIT
+    # devices that cannot host the persistent kernel run batch-1 greedy decoding on the per-phase kernels
+    mega = B == 1 and not args.sampling and not (flags & capi.GEN_NO_MEGA) and \
+        capi.lib().ma_decode_persistent_supported() == 1
     pc_host = synthetic_pc_normal(B, first=rank * B).pin_memory()     # fp16 [B,4096,6]
     pc_dev = pc_host.to(dev)
     _, prefix_dev = model.point_encoder.encode_with_prefix(pc_dev)
@@ -353,12 +376,14 @@ def main():
     ms, out = timed(one_step_resident, args.steps)
     clocks = sampler.stop()
     launches = capi.lib().ma_launch_count() - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"meshes": out})
     ms_e2e, out_e2e = timed(one_step_e2e, args.steps)
     e2e_remeasured = None
     if ms_e2e > 1.5 * ms:   # the e2e pass only adds ~50 KB of copies: a large gap is a disturbed measurement, not the path
         e2e_remeasured = ms_e2e
         ms_e2e, out_e2e = timed(one_step_e2e, args.steps)
-    mega_err = gen.mega_error() if (B == 1 and not args.sampling) else 0
+    mega_err = gen.mega_error() if mega else 0
     # stage split of one pass (encoder / decode loop / detokenizer), device timed
     if args.lean:
         ms_enc, ms_gen, gen_out = 0.0, ms, (model.last_ids,)
@@ -399,21 +424,14 @@ def main():
     t_prefill_ms = t100 - (n_lo - 1) * us_step_short / 1000.0
     dec_ms = ms / args.steps - max(0.0, t_prefill_ms)             # decode-loop part of one generate
     achieved = alg_bytes_per_gen / (dec_ms / 1000.0) / 1e9
-    traffic = None   # DRAM bytes per decode token from the committed ncu --set full capture of the same kernel
-    for tag in ("r02", "r01"):     # the newest committed `ncu --set full` capture of the persistent kernel
-        tpath = os.path.join(ROOT, "profiles", f"traffic_{tag}.json")
-        if B == 1 and not args.sampling and os.path.exists(tpath):
-            traffic = json.load(open(tpath))["traffic_bytes_per_token"]
-            break
     roofline = {
         "bound": "hbm",
         "kernel": ("decode_mega_kernel (persistent: all 121 phases of a token, 512 tokens per launch)"
-                   if (B == 1 and not args.sampling and not (flags & capi.GEN_NO_MEGA)) else
+                   if mega else
                    "decode step = 97 fast_gemv_kernel + 24 attention_kernel launches (one CUDA graph)" if B == 1 else
-                   "decode step: gemm_ws_kernel (tcgen05 swap-AB, K slices in a cluster) + attention_stream_kernel + sample_kernel, one CUDA graph"
+                   "decode step: gemm_ws_kernel (wgmma swap-AB, K slices in a cluster) + attention_stream_kernel + sample_kernel, one CUDA graph"
                    if args.sampling else "decode step (gemm_canon + attention kernels, one CUDA graph)"),
         "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "peak_source": peak_src,
-        "traffic": traffic,
         "algorithmic_bytes_per_launch": alg_bytes_per_gen / n_dec,
         "launch": "one decode step (one token of every sequence); bytes = fp16 weights %d + KV read/write averaged over the run" % wbytes,
         "us_per_step_avg": dec_ms * 1000.0 / n_dec,
@@ -449,7 +467,7 @@ def main():
                        "inputs": "pc_normal fp16 [B,4096,6] resident in HBM; one step = encoder + generate + detokenize",
                        "stage_ms": {"encoder": ms_enc / args.steps, "generate": ms_gen / args.steps,
                                     "detokenize_and_rest": max(0.0, (ms_all - ms_enc - ms_gen) / args.steps)},   # separate runs: noise can exceed it
-                       "l2": "inputs larger than L2: 623.5 MB of weights + KV streamed per token (L2 = 126 MB)",
+                       "l2": "inputs larger than L2: 623.5 MB of weights + KV streamed per token (L2 = 50 MB)",
                        "checkpoint": "synthetic seed 0 (random weights: no early EOS, every sequence runs the cap)"},
             "roofline": roofline, "cpu_baseline": cpu,
             "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": int(pc_host.numel() * 2),

@@ -1,5 +1,5 @@
 /*
- * meshanything_b200.h -- C ABI of libmeshanything_b200.so (sm_100a).
+ * meshanything_b200.h -- C ABI of libmeshanything_b200.so (sm_90a, H100).
  *
  * The reference (buaacyw/MeshAnything) exposes no FFI: its boundary is the Python surface
  * (SURVEY.md section 8b).  These entry points are the seams inside `MeshAnything.forward`
@@ -161,7 +161,7 @@ int ma_decode_slots_poll(int B, int tmax, void* ws, int32_t* finished_host, int3
 #define MA_GEN_NO_PDL 4     /* batch-1 fast path without programmatic dependent launch */
 #define MA_GEN_NO_EARLY_EXIT 8
 #define MA_GEN_NO_MEGA 16    /* batch-1 greedy: per-phase kernels (decode_fast.cu) instead of the persistent kernel */
-#define MA_GEN_TC 64         /* batches: decoder GEMMs on the tensor cores (tcgen05) -- logits within a tolerance of the
+#define MA_GEN_TC 64         /* batches: decoder GEMMs on the tensor cores (wgmma) -- logits within a tolerance of the
                                 canonical kernels instead of bit-exact ids; implied by sampling */
 #define MA_GEN_TRACE 32      /* persistent kernel records globaltimer stamps of CTA 0 at every phase boundary */
 
@@ -172,14 +172,19 @@ int ma_decoder_debug(void* ws, int B, int tmax, int what, void* host_out, int nb
 /* Test hook of the persistent kernel: bound of every in-kernel wait in ns (0 = keep; default: seconds) and fault
  * injection (fault = c + 1: CTA c withholds its out_proj rows from the third token on, so the hand-off times out). */
 void ma_mega_set_debug(unsigned long long timeout_ns, int fault);
+/* 1 if the persistent kernel can run on the current device (then batch-1 greedy decoding uses it unless
+ * MA_GEN_NO_MEGA is set), 0 if batch-1 greedy decoding always takes the per-phase kernels there.  The kernel needs
+ * every CTA to own fc1 and lm_head rows (at most 64 of each), the last 16 CTAs to own no out_proj rows, and a CTA's
+ * rows to fit its shared memory: 147 SMs do, the 132 of an H100 do not. */
+int ma_decode_persistent_supported(void);
 
 
-/* Same contract as ma_linear_f16 on the tcgen05 tensor cores (TMA-fed, accumulator in TMEM): fp16 in, fp32
+/* Same contract as ma_linear_f16 on the wgmma tensor cores (TMA-fed, fp32 accumulator in registers): fp16 in, fp32
  * accumulate in the hardware's order (NOT the canonical order: results agree with ma_linear_f16 to fp32 rounding,
  * not bit for bit).  M >= 64, N % 128 == 0, K % 64 == 0.  Used by ma_encoder_forward / ma_detokenize. */
 int ma_linear_tc_f16(const void* W, const void* bias, const void* x, int ldx, void* y, int ldy, int M, int N, int K,
                      int epilogue, void* stream);
-/* The same contract for FEW rows (1 <= M <= 128; any N; K % 64 == 0): swap-AB weight-streaming tcgen05 GEMM with the K
+/* The same contract for FEW rows (1 <= M <= 128; any N; K % 64 == 0): swap-AB weight-streaming wgmma GEMM with the K
  * dimension split across CTAs and a deterministic last-CTA reduction (gemm_ws.cu).  Replaces the cuBLAS GEMMs of HF's
  * OPTDecoderLayer for a decode step of a batch (shape_opt.py:403-410).  scratch: ma_linear_ws_scratch_bytes() bytes,
  * zero-filled once by the caller.  Hardware accumulation order: compared under a tolerance. */
@@ -192,11 +197,11 @@ int ma_linear_ws_f16(const void* W, const void* bias, const void* x, int ldx, vo
 /* 0: canonical CUDA-core kernels everywhere; 1: encoder / detokenizer GEMMs on the tensor cores; 2: their attention
  * too (ma_attention_tc_f16).  Returns the previous setting. */
 int ma_set_tensor_cores(int enable);
-/* Linear calls of ma_encoder_forward / ma_detokenize since load: how many ran on tcgen05 and how many fell back to the
+/* Linear calls of ma_encoder_forward / ma_detokenize since load: how many ran on the tensor cores and how many fell back to the
  * canonical CUDA-core kernel because their shape cannot be tiled (M < 64, N % 128 != 0). */
-void ma_tensor_core_linear_counts(unsigned long long* on_tcgen05, unsigned long long* canonical_fallback);
+void ma_tensor_core_linear_counts(unsigned long long* on_tensor_cores, unsigned long long* canonical_fallback);
 
-/* Dense non-causal attention on the tensor cores (tcgen05 flash attention; replaces F.scaled_dot_product_attention of
+/* Dense non-causal attention on the tensor cores (wgmma flash attention; replaces F.scaled_dot_product_attention of
  * transformer_blocks.py:57-74,166-185 and BERT's attention in meshanything.py:62-64).  q fp16 [n_slots*rows_per_slot][ldq]
  * (head h at columns 64h..64h+63), K fp16 [n_slots][H][T][64], Vt fp16 [n_slots][H][64][Tpad] = V transposed, zero for
  * keys >= nkeys, Tpad a multiple of 64 and >= nkeys rounded up to 128; every query of a slot sees the first nkeys

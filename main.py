@@ -1,4 +1,4 @@
-"""Drop-in for /root/reference/main.py (same flags, same outputs) on top of the B200-native MeshAnything.
+"""Drop-in for /root/reference/main.py (same flags, same outputs) on top of the H100-native MeshAnything.
 
     python main.py --input_type pc_normal --input_path pc_examples/mouse.npy --out_dir out [--sampling]
     torchrun --nproc-per-node 8 main.py --input_type pc_normal --input_dir pcs --batchsize_per_gpu 64

@@ -1,4 +1,4 @@
-"""Builds libmeshanything_b200.so in-tree with nvcc for sm_100a (no JIT cache: the .so travels to the GPU box)."""
+"""Builds libmeshanything_b200.so in-tree with nvcc for sm_90a (H100); no JIT cache, the library lives in the tree."""
 from __future__ import annotations
 
 import os
@@ -10,15 +10,10 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
-# MA_B200_NO_FHFMA=1 selects the convert + FFMA variant of the canonical dot products (own file names, so both builds
-# travel to the GPU box side by side); the default uses the mixed-precision FMA (SASS FHFMA), see canon.cuh
-VARIANT = "_nofhfma" if os.environ.get("MA_B200_NO_FHFMA") == "1" else ""
-LIB = os.path.join(LIB_DIR, f"libmeshanything_b200{VARIANT}.so")
+LIB = os.path.join(LIB_DIR, "libmeshanything_b200.so")
 SOURCES = ["gemm_canon.cu", "attention.cu", "attention_stream.cu", "elementwise.cu", "decode_fast.cu", "decode_mega.cu", "api.cu", "glue.cu", "gemm_tc.cu", "gemm_ws.cu", "attention_tc.cu", "api_encoder.cu", "surface.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
-if VARIANT:
-    NVCC_FLAGS.append("-DMA_NO_FHFMA")
 
 
 def _nvcc() -> str:
@@ -52,7 +47,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
     objs = []
 
     def compile_one(src: str) -> str:
-        obj = os.path.join(LIB_DIR, src.replace(".cu", f"{VARIANT}.o"))
+        obj = os.path.join(LIB_DIR, src.replace(".cu", ".o"))
         cmd = [nvcc, *NVCC_FLAGS, "-ccbin", "g++", "-c", os.path.join(CSRC, src), "-o", obj]
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
@@ -65,7 +60,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
     with ThreadPoolExecutor(max_workers=len(SOURCES)) as ex:
         objs = list(ex.map(compile_one, SOURCES))
-    cmd = [nvcc, "-shared", "-ccbin", "g++", "-o", LIB, *objs, "-lcudart"]
+    cmd = [nvcc, "-shared", *NVCC_FLAGS[:2], "-ccbin", "g++", "-o", LIB, *objs, "-lcudart"]
     r = subprocess.run(cmd, capture_output=True, text=True, env=env)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

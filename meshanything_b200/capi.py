@@ -1,6 +1,6 @@
 """ctypes binding of libmeshanything_b200.so (include/meshanything_b200.h).
 
-The library is built in-tree by `meshanything_b200.build` (nvcc, sm_100a).  There is no CPU or
+The library is built in-tree by `meshanything_b200.build` (nvcc, sm_90a).  There is no CPU or
 PyTorch fallback: if the shared object cannot be loaded every call raises.
 """
 from __future__ import annotations
@@ -44,7 +44,7 @@ EXPORTS = [
     "ma_attention_tc_f16", "ma_transpose_heads_f16",
     "ma_decode_slots_init", "ma_decode_slot_prefill", "ma_decode_slots_step", "ma_decode_slots_poll",
     "ma_mega_set_debug", "ma_linear_ws_set_mode", "ma_decode_slots_seek", "ma_decode_slot_stream", "ma_linear_ws_scratch_bytes", "ma_linear_ws_f16",
-    "ma_sample_surface_workspace_bytes", "ma_sample_surface", "ma_tensor_core_linear_counts",
+    "ma_sample_surface_workspace_bytes", "ma_sample_surface", "ma_tensor_core_linear_counts", "ma_decode_persistent_supported",
 ]
 
 
@@ -100,6 +100,8 @@ def lib():
     L.ma_decoder_debug.argtypes = [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int]
     L.ma_mega_set_debug.argtypes = [C.c_ulonglong, C.c_int]
     L.ma_mega_set_debug.restype = None
+    L.ma_decode_persistent_supported.argtypes = []
+    L.ma_decode_persistent_supported.restype = C.c_int
     L.ma_encoder_workspace_bytes.argtypes = [C.c_int]
     L.ma_encoder_workspace_bytes.restype = C.c_size_t
     L.ma_encoder_forward.argtypes = [_vp, _vp, C.c_int, _vp, _vp, _vp, _vp]
@@ -173,7 +175,7 @@ def sample_surface(vertices: torch.Tensor, faces: torch.Tensor, n_samples: int, 
 
 
 def tensor_core_linear_counts():
-    """(Linear calls of the encoder / detokenizer that ran on tcgen05, calls that fell back to the canonical kernel)."""
+    """(Linear calls of the encoder / detokenizer that ran on the tensor cores, calls that fell back to the canonical kernel)."""
     a, b = C.c_ulonglong(0), C.c_ulonglong(0)
     lib().ma_tensor_core_linear_counts(C.byref(a), C.byref(b))
     return a.value, b.value
@@ -183,7 +185,7 @@ _ws_scratch = {}
 
 
 def linear_ws_f16(w: torch.Tensor, bias: Optional[torch.Tensor], x: torch.Tensor, epilogue: int = EPI_NONE) -> torch.Tensor:
-    """fp16(x @ w.T + bias) for M <= 128 rows on the weight-streaming tcgen05 GEMM (hardware accumulation order)."""
+    """fp16(x @ w.T + bias) for M <= 128 rows on the weight-streaming wgmma GEMM (hardware accumulation order)."""
     _need_cuda(w, bias, x)
     M, K = x.shape
     N = w.shape[0]
@@ -197,7 +199,7 @@ def linear_ws_f16(w: torch.Tensor, bias: Optional[torch.Tensor], x: torch.Tensor
 
 
 def linear_tc_f16(w: torch.Tensor, bias: Optional[torch.Tensor], x: torch.Tensor, epilogue: int = EPI_NONE) -> torch.Tensor:
-    """fp16(x @ w.T + bias) on the tcgen05 tensor cores (hardware accumulation order)."""
+    """fp16(x @ w.T + bias) on the wgmma tensor cores (hardware accumulation order)."""
     _need_cuda(w, bias, x)
     M, K = x.shape
     N = w.shape[0]
@@ -220,7 +222,7 @@ def transpose_heads_f16(src: torch.Tensor, col0: int, head_stride: int, H: int, 
 def attention_tc_f16(q: torch.Tensor, k: torch.Tensor, vt: torch.Tensor, nkeys: int, rows_per_slot: int,
                      scale: float = 0.125) -> torch.Tensor:
     """q [n_slots*rows_per_slot, H*64]; k [n_slots, H, T, 64]; vt [n_slots, H, 64, Tpad] (V transposed, zero beyond
-    nkeys) -> [rows, H*64], on the tcgen05 tensor cores."""
+    nkeys) -> [rows, H*64], on the wgmma tensor cores."""
     _need_cuda(q, k, vt)
     S, H, T, _ = k.shape
     Tpad = vt.shape[3]

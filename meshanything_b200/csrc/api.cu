@@ -110,14 +110,13 @@ static const bool g_no_pdl = [] {   // MA_B200_NO_PDL=1: plain stream order betw
 
 // One pass of the 24 layers over M rows (general batched kernels).
 // y = act(x W^T + b) for M rows of the decoder: the canonical kernel, or (tc) the tensor cores -- the weight-streaming
-// tcgen05 GEMM for M <= 128 rows (decode steps), the tiled tcgen05 GEMM for the 257-row prefill passes
+// wgmma GEMM for M <= 128 rows (decode steps), the tiled wgmma GEMM for the 257-row prefill passes
 static int dec_linear(bool tc, const DecWs& ws, const void* W, const void* b, const __half* x, int ldx, __half* y, int ldy,
                       int M, int N, int K, int epi, cudaStream_t st, bool pdl = false) {
   if (tc) {
-    // measured at M = 64 (profiles/batched_kernels_r02.json, us per call; tiled gemm_tc / weight-streaming with the K
-    // slices in a cluster / the same with L2 tickets): qkv 9.2 / 7.5 / 11.4, out_proj 7.3 / 6.1 / 15.7, fc1 9.4 / 8.1 /
-    // 11.6, fc2 22.7 / 8.2 / 18.8, lm_head - / 10.4 / 12.2 (N = 8195 is not tileable; canonical kernel 42.7).  So up to
-    // 128 rows the cluster kernel takes every matrix; the tiled kernel keeps the 257-row prefill passes.
+    // Up to 128 rows the weight-streaming kernel takes every matrix (it reads each weight once and splits K across
+    // the SMs; lm_head, N = 8195, is not tileable at all); the tiled kernel keeps the 257-row prefill passes.
+    // tools/bench_batched.py times the three kernels per decoder shape.
     const bool tiled_ok = M >= 64 && linear_tc_supported(M, N, K, ldx, ldy, x, W, y);
     const bool ws_ok = M <= 128 && linear_ws_supported(M, N, K, ldx, x, W);
     if (ws_ok && (linear_ws_mode() || !tiled_ok || K > 1024))
@@ -627,10 +626,15 @@ int ma_decode_slots_poll(int B, int tmax, void* ws_, int32_t* finished_host, int
 
 
 void ma_mega_set_debug(unsigned long long timeout_ns, int fault) { mega_set_debug(timeout_ns, fault); }
+int ma_decode_persistent_supported(void) { return mega_supported(); }
 
 int ma_decoder_debug(void* ws_, int B, int tmax, int what, void* host_out, int nbytes) {
   DecWs ws = carve(ws_, B, tmax, 8195 + 61);
   cudaDeviceSynchronize();
+  if (what == 0 && !mega_supported()) {   // the persistent kernel never runs on this device: nothing can time out
+    memset(host_out, 0, (size_t)nbytes);
+    return 0;
+  }
   const char* src = (const char*)ws.mega + (what == 0 ? mega_error_flag_offset() : what == 1 ? mega_trace_offset() : mega_trace_cta_offset());
   return cudaMemcpy(host_out, src, (size_t)nbytes, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : 1;
 }

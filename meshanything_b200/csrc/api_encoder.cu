@@ -69,11 +69,11 @@ static EncWs carve_enc(void* base, int Bc) {
 
 #define TRY(x) do { if (x) return 1; } while (0)
 
-static int g_use_tc = 2;  // 0: canonical CUDA-core kernels; 1: GEMMs of the encoder / detokenizer on tcgen05;
-                          // 2: their attention on tcgen05 too (ma_set_tensor_cores)
+static int g_use_tc = 2;  // 0: canonical CUDA-core kernels; 1: GEMMs of the encoder / detokenizer on the tensor cores;
+                          // 2: their attention on the tensor cores too (ma_set_tensor_cores)
 
 // nn.Linear of the tolerance-checked stages: tensor cores when the shape allows, canonical CUDA-core kernel otherwise
-static unsigned long long g_tc_calls = 0, g_tc_fallbacks = 0;   // Linear calls of these stages: on tcgen05 / not tileable
+static unsigned long long g_tc_calls = 0, g_tc_fallbacks = 0;   // Linear calls of these stages: on the tensor cores / not tileable
 static int enc_linear(const __half* W, const __half* bias, const __half* x, int ldx, __half* y, int ldy, int M, int N,
                       int K, int epi, cudaStream_t st) {
   if (g_use_tc && linear_tc_supported(M, N, K, ldx, ldy, x, W, y)) {
@@ -86,7 +86,7 @@ static int enc_linear(const __half* W, const __half* bias, const __half* x, int 
 
 // Dense attention of n_slots x rows_per_slot queries over the n keys of their slot.  q [rows][ldq] (head h at 64h), kh
 // [slot][H][n][64] already scattered; V is still in its source matrix (vsrc, vld, vcol0, vstride as for
-// scatter_heads) and is laid out here the way the chosen kernel wants it: transposed + zero-padded for tcgen05, head-
+// scatter_heads) and is laid out here the way the chosen kernel wants it: transposed + zero-padded for the tensor-core attention, head-
 // major for the canonical kernel.
 static int enc_attention(const __half* q, int ldq, const __half* kh, const __half* vsrc, int vld, int vcol0,
                          int vstride, __half* vbuf, int n, int rows_per_slot, int n_slots, const int* nkeys,
@@ -207,7 +207,7 @@ static DetWs carve_det(void* base, int Bc, int F) {
   w.qkv16 = c.take<__half>(R * 3 * EW);
   w.qh = c.take<__half>(R * EW);
   w.kh = c.take<__half>(R * EW);
-  w.vh = c.take<__half>((size_t)Bc * ((S + 127) / 128 * 128) * EW);  // room for V^T padded to 128 keys (tcgen05 path)
+  w.vh = c.take<__half>((size_t)Bc * ((S + 127) / 128 * 128) * EW);  // room for V^T padded to 128 keys (tensor-core path)
   w.attn16 = c.take<__half>(R * EW);
   w.y16 = c.take<__half>(R * EW);
   w.f16 = c.take<__half>(R * 4 * EW);
@@ -277,8 +277,8 @@ using namespace ma;
 
 extern "C" {
 
-void ma_tensor_core_linear_counts(unsigned long long* on_tcgen05, unsigned long long* canonical_fallback) {
-  if (on_tcgen05) *on_tcgen05 = g_tc_calls;
+void ma_tensor_core_linear_counts(unsigned long long* on_tensor_cores, unsigned long long* canonical_fallback) {
+  if (on_tensor_cores) *on_tensor_cores = g_tc_calls;
   if (canonical_fallback) *canonical_fallback = g_tc_fallbacks;
 }
 

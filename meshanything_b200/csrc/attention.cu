@@ -89,15 +89,11 @@ __global__ void __launch_bounds__(ATT_THREADS) attention_kernel(AttnArgs a) {
       bulk_g2s(sm.v + len_early * HD, a.V + base + (long)len_early * HD, rest * HD * 2, &sm.bar[1]);
     }
   }
-#ifdef MA_FHFMA
-  const uint4 qp = *reinterpret_cast<const uint4*>(a.q + (long)m * a.ldq + h * HD + 8 * li);  // stays packed (FHFMA)
-#else
   float qf[8];
   {
     uint4 u = *reinterpret_cast<const uint4*>(a.q + (long)m * a.ldq + h * HD + 8 * li);
     unpack8(u, qf);
   }
-#endif
   __syncthreads();  // barrier inits visible to all waiters
   if (len_early > 0) mbar_wait(&sm.bar[0], 0);
   if (len - len_early > 0) mbar_wait(&sm.bar[1], 0);
@@ -109,15 +105,11 @@ __global__ void __launch_bounds__(ATT_THREADS) attention_kernel(AttnArgs a) {
     const int r = 32 * rho + 4 * warp + grp;
     const int rr = min(r, len - 1);
     uint4 u = *reinterpret_cast<const uint4*>(sm.k + rr * HD + 8 * li);
-#ifdef MA_FHFMA
-    float p = dot8_packed(qp, u, 0.0f);
-#else
     float kf[8];
     unpack8(u, kf);
     float p = 0.0f;
 #pragma unroll
     for (int j = 0; j < 8; j++) p = ffma(qf[j], kf[j], p);
-#endif
     p = fadd(p, __shfl_xor_sync(0xffffffffu, p, 4));
     p = fadd(p, __shfl_xor_sync(0xffffffffu, p, 2));
     p = fadd(p, __shfl_xor_sync(0xffffffffu, p, 1));
@@ -145,21 +137,11 @@ __global__ void __launch_bounds__(ATT_THREADS) attention_kernel(AttnArgs a) {
       const float e = ma_exp(fsub(sm.s[r], cmax));
       l = fadd(l, e);
       uint4 u = *reinterpret_cast<const uint4*>(sm.v + r * HD + 8 * li);
-#ifdef MA_FHFMA
-      const unsigned short ph = __half_as_ushort(__float2half_rn(e));
-      const uint32_t vw[4] = {u.x, u.y, u.z, u.w};
-#pragma unroll
-      for (int i = 0; i < 4; i++) {
-        o[2 * i] = fhfma(ph, (unsigned short)(vw[i] & 0xffffu), o[2 * i]);
-        o[2 * i + 1] = fhfma(ph, (unsigned short)(vw[i] >> 16), o[2 * i + 1]);
-      }
-#else
       const float pf = __half2float(__float2half_rn(e));
       float vf[8];
       unpack8(u, vf);
 #pragma unroll
       for (int j = 0; j < 8; j++) o[j] = ffma(pf, vf[j], o[j]);
-#endif
     }
   }
   // groups of the warp: (g0+g2)+(g1+g3)

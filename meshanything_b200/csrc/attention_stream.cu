@@ -4,7 +4,7 @@
 // for q [B,1,16,64] against the KV cache, /root/reference/MeshAnything/models/shape_opt.py:205 -> transformers'
 // OPTDecoderLayer attention) -- bit for bit: same chunks of MA_ATTN_CHUNK keys, same lane chains, same butterflies,
 // same ascending merge.  What changes is how the bytes move.  attention_kernel gives every (row, head, chunk) its own
-// CTA that loads 64 KB, waits for all of it, computes and exits (5.0 TB/s on a batch of 64, profiles/batched_kernels).
+// CTA that loads 64 KB, waits for all of it, computes and exits.
 // Here two persistent CTAs per SM each walk their share of the work; a work item is a SEGMENT = a few consecutive
 // chunks of one (row, head):
 //   * warp 0 is the producer: the K rows and the V rows of a chunk are two 32 KB half-stages of a 3-slot ring
@@ -307,7 +307,7 @@ int launch_attention_decode(const __half* qkv, int ldq, __half* K, __half* V, lo
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     cudaFuncSetAttribute(attention_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
                          (int)sizeof(AttnStreamSmem));
-    g_as_ctas = 2 * (sms > 0 ? sms : 148);   // two CTAs per SM
+    g_as_ctas = 2 * (sms > 0 ? sms : 132);   // two CTAs per SM
   }
   const int chunks = (max_keys + MA_ATTN_CHUNK - 1) / MA_ATTN_CHUNK;
   AttnStreamArgs a;

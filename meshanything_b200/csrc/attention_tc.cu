@@ -1,34 +1,32 @@
-// attention_tc.cu -- dense (non-causal) attention softmax(q K^T * scale) V on the 5th-generation tensor cores, for the
+// attention_tc.cu -- dense (non-causal) attention softmax(q K^T * scale) V on the Hopper tensor cores, for the
 // stages compared under a tolerance: the Perceiver cross-attention (257 queries x 4096 keys x 12 heads,
 // transformer_blocks.py:166-185), the 24 Michelangelo self-attention layers (:57-74) and the 6 BERT layers of the
 // detokenizer (meshanything.py:50-80).  The decoder keeps the canonical CUDA-core attention (DESIGN.md section 3).
 //
-// One CTA = 128 queries of one (slot, head); loop over blocks of 128 keys (flash-attention recurrence):
-//   S = Q K_j^T          tcgen05.mma M128 N128 K16 x4   (Q, K_j: K-major tiles [128][64 halfs], TMA, 128-byte swizzle)
-//   P = exp2((S - m) * scale * log2 e)  one thread per query row: tcgen05.ld of its S row from TMEM, running max /
-//                        sum, P rounded to fp16 and stored to shared memory in the same swizzled K-major layout
-//   O_j = P V_j          tcgen05.mma M128 N64 K16 x8    (P: two [128][64] tiles; V_j^T: two [64 d][64 keys] tiles --
-//                        V is kept TRANSPOSED in global memory ([slot][head][64][Tpad]) so that it is K-major too)
-//   O = O * alpha + O_j  in registers (64 fp32 per thread), so nothing in TMEM is ever rescaled
-// 192 threads: warps 0-3 softmax/epilogue (TMEM lane quadrant = warp), warp 4 MMA issuer + TMEM allocator,
-// warp 5 TMA producer.  K/V^T double-buffered; S (128 columns) and O_j (64 columns) live in one 256-column TMEM
-// allocation.  mbarriers: q_full, kv_full/kv_empty[2], s_full, p_full (128 arrivals), o_full, o_empty (128).
+// One CTA = 128 queries of one (slot, head); loop over blocks of 128 keys (flash-attention recurrence).  Consumer
+// warpgroup g (warps 4g .. 4g+3) owns query rows 64g .. 64g+63:
+//   S = Q K_j^T          wgmma m64n128k16 x4 from shared memory (Q, K_j: K-major tiles [rows][64 halfs], TMA, 128-byte
+//                        swizzle); S stays in registers (a thread holds 2 rows x 32 columns)
+//   P = exp2((S - m) * scale * log2 e)  running max / sum per row over the 4 threads of a quad, P rounded to fp16
+//                        and packed in registers in the A-operand layout of the next wgmma
+//   O = O * alpha + P V_j  wgmma m64n64k16 x8 with A = P from registers, B = V_j^T from shared memory (two
+//                        [64 d][64 keys] tiles; V is kept TRANSPOSED in global memory ([slot][head][64][Tpad]) so that
+//                        it is K-major too)
+// 288 threads: warps 0-7 the two consumer warpgroups, warp 8 TMA producer.  K/V^T double-buffered; mbarriers q_full,
+// kv_full[2] (TMA transactions), kv_empty[2] (one arrival per consumer warp).
 #include "internal.h"
 #include "tc_common.cuh"
 
 namespace ma {
 
-constexpr int FA_BQ = 128, FA_BK = 128, FA_STAGES = 2, FA_THREADS = 192;
-constexpr uint32_t FA_TMEM_COLS = 256, FA_S_COL = 0, FA_O_COL = 128;
+constexpr int FA_BQ = 128, FA_BK = 128, FA_STAGES = 2, FA_THREADS = 288, FA_CONSUMER_WARPS = 8;
 constexpr uint32_t FA_SPIN_LIMIT = 1u << 27;  // bounded polls (a few seconds): a protocol bug traps instead of hanging the GPU
 
 struct alignas(1024) FaSmem {
   __half q[FA_BQ * 64];                   // 16 KB
   __half k[FA_STAGES][FA_BK * 64];        // 16 KB each
   __half vt[FA_STAGES][2][64 * 64];       // per stage: V^T for keys 0..63 and 64..127 of the block, 8 KB each
-  __half p[2][FA_BQ * 64];                // P tile, keys 0..63 | 64..127
-  uint64_t q_full, kv_full[FA_STAGES], kv_empty[FA_STAGES], s_full, p_full, o_full, o_empty;
-  uint32_t tmem_base;
+  uint64_t q_full, kv_full[FA_STAGES], kv_empty[FA_STAGES];
 };
 
 __device__ __forceinline__ void fa_wait(uint64_t* bar, uint32_t parity) {
@@ -46,6 +44,11 @@ __device__ __forceinline__ void fa_wait(uint64_t* bar, uint32_t parity) {
   __trap();
 }
 
+__device__ __forceinline__ uint32_t pack_half2(__half lo, __half hi) {
+  __half2 v = __halves2half2(lo, hi);
+  return *reinterpret_cast<uint32_t*>(&v);
+}
+
 struct FaArgs {
   __half* out;
   int ldo, H, rows_per_slot, nkeys;
@@ -59,43 +62,30 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   FaSmem& sm = *reinterpret_cast<FaSmem*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int qt = blockIdx.x, h = blockIdx.y, slot = blockIdx.z;
+  const int qt = blockIdx.x, hd = blockIdx.y, slot = blockIdx.z;
   const int row0 = slot * a.rows_per_slot + qt * FA_BQ;          // first query row of this tile (global row index)
   const int valid_rows = min(FA_BQ, a.rows_per_slot - qt * FA_BQ);
   const int nb = (a.nkeys + FA_BK - 1) / FA_BK;
-  const long head = (long)slot * a.H + h;
+  const long head = (long)slot * a.H + hd;
 
-  if (warp == 5 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_k) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_vt) : "memory");
+  if (threadIdx.x == 0) {
     mbar_init(&sm.q_full, 1);
     for (int s = 0; s < FA_STAGES; s++) {
       mbar_init(&sm.kv_full[s], 1);
-      mbar_init(&sm.kv_empty[s], 1);
+      mbar_init(&sm.kv_empty[s], FA_CONSUMER_WARPS);
     }
-    mbar_init(&sm.s_full, 1);
-    mbar_init(&sm.p_full, FA_BQ);
-    mbar_init(&sm.o_full, 1);
-    mbar_init(&sm.o_empty, FA_BQ);
     mbar_fence_init();
   }
-  if (warp == 4) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sm.tmem_base)),
-                 "n"(FA_TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = sm.tmem_base;
 
-  if (warp == 5) {
+  if (warp == FA_CONSUMER_WARPS) {
     // ---------------- TMA producer
     if (elect_one()) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_q) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_k) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_vt) : "memory");
       mbar_expect_tx(&sm.q_full, FA_BQ * 64 * 2);
-      tma_load_2d(sm.q, &map_q, 64 * h, row0, &sm.q_full);
+      tma_load_2d(sm.q, &map_q, 64 * hd, row0, &sm.q_full);
       for (int j = 0; j < nb; j++) {
         const int s = j % FA_STAGES;
         const uint32_t ph = (j / FA_STAGES) & 1;
@@ -106,123 +96,94 @@ __global__ void __launch_bounds__(FA_THREADS, 1)
         tma_load_2d(sm.vt[s][1], &map_vt, j * FA_BK + 64, (int)(head * 64), &sm.kv_full[s]);
       }
     }
-  } else if (warp == 4) {
-    // ---------------- MMA issuer.  idesc: D=f32, A=B=f16, both K-major, N>>3 at bit 17, M>>4 at bit 24
-    constexpr uint32_t idesc_qk = (1u << 4) | ((uint32_t)(FA_BK >> 3) << 17) | ((uint32_t)(FA_BQ >> 4) << 24);
-    constexpr uint32_t idesc_pv = (1u << 4) | ((uint32_t)(64 >> 3) << 17) | ((uint32_t)(FA_BQ >> 4) << 24);
-    auto issue_qk = [&](int s) {
-      const uint64_t ad = umma_desc(sm.q), bd = umma_desc(sm.k[s]);
-#pragma unroll
-      for (int k = 0; k < 4; k++) umma_f16(tmem + FA_S_COL, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), idesc_qk, k ? 1u : 0u);
-      umma_commit(&sm.s_full);
-    };
-    fa_wait(&sm.q_full, 0);
-    fa_wait(&sm.kv_full[0], 0);
-    tc_fence_after();
-    if (elect_one()) issue_qk(0);
-    __syncwarp();
-    for (int j = 0; j < nb; j++) {
-      const int s = j % FA_STAGES;
-      fa_wait(&sm.p_full, j & 1);                    // P_j is in shared memory, S_j has been consumed
-      if (j > 0) fa_wait(&sm.o_empty, (j - 1) & 1);  // O_{j-1} has been read out of TMEM
-      tc_fence_after();
-      if (elect_one()) {
-#pragma unroll
-        for (int kk = 0; kk < 8; kk++) {
-          const uint64_t ad = umma_desc(sm.p[kk >> 2]) + (uint64_t)((kk & 3) * 2);
-          const uint64_t bd = umma_desc(sm.vt[s][kk >> 2]) + (uint64_t)((kk & 3) * 2);
-          umma_f16(tmem + FA_O_COL, ad, bd, idesc_pv, kk ? 1u : 0u);
-        }
-        umma_commit(&sm.o_full);       // O_j complete (also: P and this K/V stage are free)
-        umma_commit(&sm.kv_empty[s]);
-      }
-      __syncwarp();
-      if (j + 1 < nb) {
-        const int s2 = (j + 1) % FA_STAGES;
-        fa_wait(&sm.kv_full[s2], ((j + 1) / FA_STAGES) & 1);
-        tc_fence_after();
-        if (elect_one()) issue_qk(s2);
-        __syncwarp();
-      }
-    }
-  } else {
-    // ---------------- softmax + output: thread = query row r of the tile = TMEM lane r
-    const int r = 32 * warp + lane;
-    const uint32_t trow = tmem + ((uint32_t)(32 * warp) << 16);
-    float m_run = -INFINITY, l_run = 0.0f;
-    float o[64];
-#pragma unroll
-    for (int i = 0; i < 64; i++) o[i] = 0.0f;
-    unsigned char* const prow0 = reinterpret_cast<unsigned char*>(sm.p[0]) + r * 128;
-    unsigned char* const prow1 = reinterpret_cast<unsigned char*>(sm.p[1]) + r * 128;
-    const int sw = r & 7;  // 128-byte swizzle: 16-byte chunk c of row r lives at chunk c ^ (r % 8)
-    for (int j = 0; j < nb; j++) {
-      const int nvalid = min(FA_BK, a.nkeys - j * FA_BK);
-      fa_wait(&sm.s_full, j & 1);
-      tc_fence_after();
-      uint32_t v[32];
-      float mx = -INFINITY;
-#pragma unroll 1
-      for (int c = 0; c < 4; c++) {
-        tmem_ld32(trow + FA_S_COL + 32 * c, v);
-#pragma unroll
-        for (int i = 0; i < 32; i++)
-          if (32 * c + i < nvalid) mx = fmaxf(mx, __uint_as_float(v[i]));
-      }
-      const float m_new = fmaxf(m_run, mx);   // nvalid >= 1, so m_new is finite
-      const float alpha = (m_run == -INFINITY) ? 0.0f : exp2f((m_run - m_new) * a.sl2);
-      float psum = 0.0f;
-      // (PV_{j-1} finished reading the P tile before this thread folded O_{j-1} in -- o_full below -- so it is free)
-#pragma unroll 1
-      for (int c = 0; c < 4; c++) {
-        tmem_ld32(trow + FA_S_COL + 32 * c, v);
-        __half ph[32];
-#pragma unroll
-        for (int i = 0; i < 32; i++) {
-          const float p = (32 * c + i < nvalid) ? exp2f((__uint_as_float(v[i]) - m_new) * a.sl2) : 0.0f;
-          ph[i] = __float2half_rn(p);
-          psum += __half2float(ph[i]);
-        }
-        // columns 32c .. 32c+31 = 16-byte chunks 4(c%2) .. 4(c%2)+3 of row r in tile c/2
-        unsigned char* base = (c < 2) ? prow0 : prow1;
-#pragma unroll
-        for (int g = 0; g < 4; g++) {
-          const int chunk = (4 * (c & 1) + g) ^ sw;
-          *reinterpret_cast<uint4*>(base + 16 * chunk) = reinterpret_cast<const uint4*>(ph)[g];
-        }
-      }
-      fence_proxy_async_smem();
-      tc_fence_before();
-      mbar_arrive(&sm.p_full);
-      l_run = l_run * alpha + psum;
-      m_run = m_new;
-      // O = O * alpha + O_j   (O_{j-1} was folded in during the previous iteration, right here)
-      fa_wait(&sm.o_full, j & 1);
-      tc_fence_after();
-#pragma unroll
-      for (int c = 0; c < 2; c++) {
-        tmem_ld32(trow + FA_O_COL + 32 * c, v);
-#pragma unroll
-        for (int i = 0; i < 32; i++) o[32 * c + i] = fmaf(o[32 * c + i], alpha, __uint_as_float(v[i]));
-      }
-      tc_fence_before();
-      mbar_arrive(&sm.o_empty);
-    }
-    if (r < valid_rows) {
-      const float inv = 1.0f / l_run;
-      __half out[64];
-#pragma unroll
-      for (int i = 0; i < 64; i++) out[i] = __float2half_rn(o[i] * inv);
-      uint4* dst = reinterpret_cast<uint4*>(a.out + (long)(row0 + r) * a.ldo + 64 * h);
-#pragma unroll
-      for (int g = 0; g < 8; g++) dst[g] = reinterpret_cast<const uint4*>(out)[g];
-    }
+    return;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(FA_TMEM_COLS) : "memory");
+  // ---------------- consumers: thread holds query rows rr and rr + 8 of the tile, key / d columns 8i + 2(lane%4) + e
+  const int g = warp >> 2;
+  const int rr = 64 * g + 16 * (warp & 3) + (lane >> 2);
+  const uint64_t qd = gmma_desc(sm.q + 64 * g * 64);
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.0f, 0.0f};
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; i++) o[i] = 0.0f;
+  fa_wait(&sm.q_full, 0);
+  for (int j = 0; j < nb; j++) {
+    const int s = j % FA_STAGES;
+    const int nvalid = min(FA_BK, a.nkeys - j * FA_BK);
+    fa_wait(&sm.kv_full[s], (j / FA_STAGES) & 1);
+    float sc[64];
+    const uint64_t kd = gmma_desc(sm.k[s]);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < 4; k++) wgmma_ss<FA_BK>(sc, qd + (uint64_t)(k * 2), kd + (uint64_t)(k * 2), k ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_reg_fence<64>(sc);
+
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int i = 0; i < 16; i++)
+#pragma unroll
+      for (int e = 0; e < 2; e++)
+        if (8 * i + 2 * (lane & 3) + e < nvalid)
+#pragma unroll
+          for (int h = 0; h < 2; h++) mx[h] = fmaxf(mx[h], sc[4 * i + 2 * h + e]);
+    float alpha[2], m_new[2], psum[2] = {0.0f, 0.0f};
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+      mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
+      m_new[h] = fmaxf(m_run[h], mx[h]);   // nvalid >= 1, so m_new is finite
+      alpha[h] = (m_run[h] == -INFINITY) ? 0.0f : exp2f((m_run[h] - m_new[h]) * a.sl2);
+    }
+    // P in the A-operand layout of wgmma: chunk kk (keys 16kk .. 16kk+15), register q = accumulator pair 8kk + 2q
+    uint32_t pa[8][4];
+#pragma unroll
+    for (int kk = 0; kk < 8; kk++)
+#pragma unroll
+      for (int q = 0; q < 4; q++) {
+        const int idx = 8 * kk + 2 * q, h = q & 1;
+        const int c = 8 * (idx >> 2) + 2 * (lane & 3);
+        __half p2[2];
+#pragma unroll
+        for (int e = 0; e < 2; e++) {
+          const float p = (c + e < nvalid) ? exp2f((sc[idx + e] - m_new[h]) * a.sl2) : 0.0f;
+          p2[e] = __float2half_rn(p);
+          psum[h] += __half2float(p2[e]);
+        }
+        pa[kk][q] = pack_half2(p2[0], p2[1]);
+      }
+#pragma unroll
+    for (int h = 0; h < 2; h++) {
+      psum[h] += __shfl_xor_sync(0xffffffffu, psum[h], 1);
+      psum[h] += __shfl_xor_sync(0xffffffffu, psum[h], 2);
+      l_run[h] = l_run[h] * alpha[h] + psum[h];
+      m_run[h] = m_new[h];
+    }
+#pragma unroll
+    for (int i = 0; i < 8; i++)
+#pragma unroll
+      for (int e = 0; e < 4; e++) o[4 * i + e] *= alpha[e >> 1];
+    wgmma_reg_fence<32>(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 8; kk++) wgmma_rs64(o, pa[kk], gmma_desc(sm.vt[s][kk >> 2]) + (uint64_t)((kk & 3) * 2));
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_reg_fence<32>(o);
+    if (lane == 0) mbar_arrive(&sm.kv_empty[s]);   // this warp is done with K_j / V_j
+  }
+#pragma unroll
+  for (int h = 0; h < 2; h++) {
+    const int r = rr + 8 * h;
+    if (r < valid_rows) {
+      const float inv = 1.0f / l_run[h];
+      __half* dst = a.out + (long)(row0 + r) * a.ldo + 64 * hd + 2 * (lane & 3);
+#pragma unroll
+      for (int i = 0; i < 8; i++)
+        *reinterpret_cast<__half2*>(dst + 8 * i) =
+            __halves2half2(__float2half_rn(o[4 * i + 2 * h] * inv), __float2half_rn(o[4 * i + 2 * h + 1] * inv));
+    }
   }
 }
 

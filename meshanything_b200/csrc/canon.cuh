@@ -47,65 +47,23 @@ __device__ __forceinline__ void unpack8(const uint4& u, float* f) {
   }
 }
 
-// Mixed-precision FMA of sm_100 (PTX fma.rn.f32.f16 -> SASS FHFMA, operands taken straight from the packed halves with
-// .H0/.H1 selectors): d = float(a) * float(b) + c with ONE rounding -- the same value as ffma(unpacked a, unpacked b, c),
-// because fp16 -> fp32 is exact -- without the 2 conversion instructions per product.  Checked on the B200 against
-// convert + FFMA on 67 M random products incl. subnormal, inf and nan inputs: 0 mismatches
-// (tools/microbench_cluster.cu, profiles/microbench_cluster_r02.txt), and by the bit-exact GPU suite against the CPU
-// oracle.  Default since round 2; -DMA_NO_FHFMA (build.py: MA_B200_NO_FHFMA=1) builds the convert + FFMA variant.
-#ifndef MA_NO_FHFMA
-#ifndef MA_FHFMA
-#define MA_FHFMA 1
-#endif
-#endif
-
-#ifdef MA_FHFMA
-__device__ __forceinline__ float fhfma(unsigned short a, unsigned short b, float c) {
-  asm("fma.rn.f32.f16 %0, %1, %2, %0;" : "+f"(c) : "h"(a), "h"(b));
-  return c;
-}
-// acc + sum_j w[j] * x[j], j = 0..7 in this order (the canonical per-lane order), on two 16-byte groups of packed halves
-__device__ __forceinline__ float dot8_packed(const uint4& w, const uint4& x, float acc) {
-  const uint32_t ww[4] = {w.x, w.y, w.z, w.w}, xw[4] = {x.x, x.y, x.z, x.w};
-#pragma unroll
-  for (int i = 0; i < 4; i++) {
-    acc = fhfma((unsigned short)(ww[i] & 0xffffu), (unsigned short)(xw[i] & 0xffffu), acc);
-    acc = fhfma((unsigned short)(ww[i] >> 16), (unsigned short)(xw[i] >> 16), acc);
-  }
-  return acc;
-}
-#endif
-
-// acc + sum_j w[j] * x[j], j = 0..7 sequentially (the canonical per-lane chain); either build gives the same bits
+// acc + sum_j w[j] * x[j], j = 0..7 sequentially (the canonical per-lane chain): fp16 -> fp32 is exact, so each
+// product-and-add is one fp32 FMA with one rounding
 __device__ __forceinline__ float dot8(const uint4& w, const uint4& x, float acc) {
-#ifdef MA_FHFMA
-  return dot8_packed(w, x, acc);
-#else
   float wf[8], xf[8];
   unpack8(w, wf);
   unpack8(x, xf);
 #pragma unroll
   for (int j = 0; j < 8; j++) acc = ffma(wf[j], xf[j], acc);
   return acc;
-#endif
 }
 // o[j] = float(p) * float(v[j]) + o[j], j = 0..7 (the P.V step of the canonical attention: P already rounded to fp16)
 __device__ __forceinline__ void pv8(__half p, const uint4& v, float* o) {
-#ifdef MA_FHFMA
-  const unsigned short ph = __half_as_ushort(p);
-  const uint32_t vw[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-  for (int i = 0; i < 4; i++) {
-    o[2 * i] = fhfma(ph, (unsigned short)(vw[i] & 0xffffu), o[2 * i]);
-    o[2 * i + 1] = fhfma(ph, (unsigned short)(vw[i] >> 16), o[2 * i + 1]);
-  }
-#else
   const float pf = __half2float(p);
   float vf[8];
   unpack8(v, vf);
 #pragma unroll
   for (int j = 0; j < 8; j++) o[j] = ffma(pf, vf[j], o[j]);
-#endif
 }
 
 __device__ __forceinline__ uint4 ldg_nc16(const void* p) {

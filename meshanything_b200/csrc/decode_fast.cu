@@ -179,14 +179,6 @@ __global__ void __launch_bounds__(FG_THREADS) fast_gemv_kernel(FastArgs a) {
     for (int i = 0; i < RB; i++) acc[i] = 0.0f;
 #pragma unroll
     for (int g = 0; g < G; g++) {
-#ifdef MA_FHFMA
-#pragma unroll
-      for (int i = 0; i < RB; i++) {
-        const int r = min(r0 + i, wn - 1);
-        const uint4 u = *reinterpret_cast<const uint4*>(sw + (size_t)(wr0 + r) * K + 256 * g + 8 * lane);
-        acc[i] = dot8_packed(u, xp[g], acc[i]);
-      }
-#else
       float xf[8];
       unpack8(xp[g], xf);
 #pragma unroll
@@ -198,7 +190,6 @@ __global__ void __launch_bounds__(FG_THREADS) fast_gemv_kernel(FastArgs a) {
 #pragma unroll
         for (int j = 0; j < 8; j++) acc[i] = ffma(wf[j], xf[j], acc[i]);
       }
-#endif
     }
 #pragma unroll
     for (int i = 0; i < RB; i++) {
@@ -328,7 +319,7 @@ int fast_step_enqueue(const ma_decoder_weights* w, SeqState s, int tmax, __half*
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_sms <= 0 || g_sms > 256) g_sms = 148;
+    if (g_sms <= 0 || g_sms > 256) g_sms = 132;
   }
   const int grid = g_sms;
   FastWs* ws = reinterpret_cast<FastWs*>(fast_ws);

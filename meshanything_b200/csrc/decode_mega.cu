@@ -16,11 +16,10 @@
 //   * the residual stream lives in shared memory; every CTA recomputes the LayerNorms redundantly.
 // Arithmetic is the canonical order of DESIGN.md section 3: results are bit-identical to
 // gemm_canon.cu / attention.cu / decode_fast.cu and to the CPU oracle.
-// Round 2 built and measured two re-partitionings of this kernel (thread-block clusters + DSMEM; 16 groups of 9 CTAs
-// with split-K out_proj / fc2 and a reducer tier: git 6b2d32b, profiles/mega_trace_r02_designB_*.txt): both were
-// slower than this row split, because every extra stage of the dependent chain costs ~1.5 us in situ whatever its
-// width (DESIGN.md section 4.1.2).  What round 2 keeps: the mixed-precision FMA (FHFMA) in every dot product, the
-// lane-transposed attention scores, the merge by every CTA at short contexts (one hand-off less), bounded waits that
+// Two re-partitionings of this kernel (thread-block clusters + DSMEM; 16 groups of 9 CTAs with split-K out_proj / fc2
+// and a reducer tier: git 6b2d32b) were slower than this row split, because every extra stage of the dependent chain
+// costs a fixed hand-off in situ whatever its width (measured on the earlier 148-SM target).  What it keeps: the lane-transposed
+// attention scores, the merge by every CTA at short contexts (one hand-off less), bounded waits that
 // surface as an error (lens = -1) instead of a silently wrong mesh, and the post-mortem record of the first time-out.
 #include "canon.cuh"
 #include "internal.h"
@@ -241,30 +240,6 @@ __device__ __forceinline__ void gemv_stage(const __half* sw, int nrows, const __
     w[i] = sw + (size_t)(has[i] ? r : warp) * K + 8 * lane;
   }
   float acc[4] = {0.0f, 0.0f, 0.0f, 0.0f};
-#ifdef MA_FHFMA
-  // FHFMA: x and the weights stay packed fp16; 8 instructions per 8 products instead of 8 + 16 conversions
-  if (!has[1]) {
-#pragma unroll 4
-    for (int g = 0; g < G; g++) {
-      const uint4 xr = *reinterpret_cast<const uint4*>(xs + 256 * g + 8 * lane);
-      acc[0] = dot8_packed(*reinterpret_cast<const uint4*>(w[0] + 256 * g), xr, acc[0]);
-    }
-  } else if (!has[2]) {
-#pragma unroll 4
-    for (int g = 0; g < G; g++) {
-      const uint4 xr = *reinterpret_cast<const uint4*>(xs + 256 * g + 8 * lane);
-      acc[0] = dot8_packed(*reinterpret_cast<const uint4*>(w[0] + 256 * g), xr, acc[0]);
-      acc[1] = dot8_packed(*reinterpret_cast<const uint4*>(w[1] + 256 * g), xr, acc[1]);
-    }
-  } else {
-#pragma unroll 2
-    for (int g = 0; g < G; g++) {
-      const uint4 xr = *reinterpret_cast<const uint4*>(xs + 256 * g + 8 * lane);
-#pragma unroll
-      for (int i = 0; i < 4; i++) acc[i] = dot8_packed(*reinterpret_cast<const uint4*>(w[i] + 256 * g), xr, acc[i]);
-    }
-  }
-#else
   if (!has[1]) {  // one row (out_proj, fc2, the tail warps of qkv / fc1)
 #pragma unroll 4
     for (int g = 0; g < G; g++) {
@@ -301,7 +276,6 @@ __device__ __forceinline__ void gemv_stage(const __half* sw, int nrows, const __
       }
     }
   }
-#endif
 #pragma unroll
   for (int i = 0; i < 4; i++) {
     if (i == 0 || has[1]) acc[i] = warp_sum(acc[i]);
@@ -546,21 +520,12 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(MegaArgs a) 
           }
         }
         // q of this head and, for the chunk that holds it, k / v of the current token: flagged words
-#ifdef MA_FHFMA
-        uint4 qp;   // q stays packed: the products below are FHFMAs on packed halves
-        {
-          uint2 d[2];
-          ll_wait_units<2>(ws->qkv_w + (h * HD + 8 * li) / 2, 1, ep, d, err);
-          qp = make_uint4(d[0].x, d[0].y, d[1].x, d[1].y);
-        }
-#else
         float qf[8];
         {
           uint2 d[2];
           ll_wait_units<2>(ws->qkv_w + (h * HD + 8 * li) / 2, 1, ep, d, err);
           unpack8(make_uint4(d[0].x, d[0].y, d[1].x, d[1].y), qf);
         }
-#endif
         if (cur >= 0 && cur < MA_ATTN_CHUNK) {
           const int rho_c = cur >> 5, gl_c = cur & 31;
           if (4 * wt + grp == gl_c) {
@@ -583,16 +548,12 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(MegaArgs a) 
         float pr[8];
 #pragma unroll
         for (int rho = 0; rho < 8; rho++) {
-#ifdef MA_FHFMA
-          pr[rho] = dot8_packed(qp, kreg[rho], 0.0f);
-#else
           float kf[8];
           unpack8(kreg[rho], kf);
           float p = 0.0f;
 #pragma unroll
           for (int j = 0; j < 8; j++) p = ffma(qf[j], kf[j], p);
           pr[rho] = p;
-#endif
         }
 #pragma unroll
         for (int sft = 4; sft >= 1; sft >>= 1) {
@@ -624,21 +585,11 @@ __global__ void __launch_bounds__(MG_THREADS, 1) decode_mega_kernel(MegaArgs a) 
           const float e = __shfl_sync(0xffffffffu, e_own, (lane & 24) | rho);   // from the lane that owns row rho
           if (r < len) {
             l = fadd(l, e);
-#ifdef MA_FHFMA
-            const unsigned short ph = __half_as_ushort(__float2half_rn(e));
-            const uint32_t vw[4] = {vreg[rho].x, vreg[rho].y, vreg[rho].z, vreg[rho].w};
-#pragma unroll
-            for (int i = 0; i < 4; i++) {
-              o[2 * i] = fhfma(ph, (unsigned short)(vw[i] & 0xffffu), o[2 * i]);
-              o[2 * i + 1] = fhfma(ph, (unsigned short)(vw[i] >> 16), o[2 * i + 1]);
-            }
-#else
             const float pf = __half2float(__float2half_rn(e));
             float vf[8];
             unpack8(vreg[rho], vf);
 #pragma unroll
             for (int j = 0; j < 8; j++) o[j] = ffma(pf, vf[j], o[j]);
-#endif
           }
         }
         l = fadd(l, __shfl_xor_sync(0xffffffffu, l, 16));
@@ -938,7 +889,7 @@ static int mega_sms() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&g_mega_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (g_mega_sms <= 0 || g_mega_sms > 160) g_mega_sms = 148;
+    if (g_mega_sms <= 0 || g_mega_sms > 160) g_mega_sms = 132;
   }
   return g_mega_sms;
 }
@@ -991,7 +942,8 @@ void mega_set_debug(unsigned long long timeout_ns, int fault) {
 }
 bool mega_fits(int tmax) { return tmax <= MAX_CHUNKS * MA_ATTN_CHUNK; }
 // Can the persistent kernel run on this device?  (every CTA must own fc1 and lm_head rows, the last 16 CTAs no
-// out_proj rows: 147 CTAs on the B200's 148 SMs)
+// out_proj rows, and a CTA's rows must fit its shared memory: at least 147 SMs.  An H100 with 132 SMs does not
+// qualify, and batch-1 greedy decoding runs on the per-phase kernels of decode_fast.cu there.)
 int mega_supported() {
   static int ok = -1;
   if (ok < 0) {

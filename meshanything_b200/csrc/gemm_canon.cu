@@ -6,7 +6,7 @@
 // the weight and activation rows, keeps R*T fp32 partial sums in registers, and the partials are
 // combined with the transposing butterfly (canon.cuh) -- 31 shuffles per 32 outputs.
 // This is CUDA-core work on purpose: the result must be bit-identical for every M (batch
-// invariance) and to the CPU oracle; DESIGN.md section 3 explains why tcgen05 cannot give that.
+// invariance) and to the CPU oracle; DESIGN.md section 3 explains why the tensor cores cannot give that.
 // SEG = 64 / 256: the segmented order of the decoder's out_proj (K = 1024) / fc2 (K = 4096) -- the order the
 // persistent decode kernel produces with its split-K partition (decode_mega.cu): every 256-wide group is reduced on
 // its own (seg 64: xor-4,2,1 inside a 64-element segment first, then the 4 segments as a tree; seg 256: the plain
@@ -88,32 +88,6 @@ __global__ void __launch_bounds__(GEMM_WARPS * 32)
     }
     return;
   }
-#ifdef MA_FHFMA
-  // FHFMA: operands stay packed (no fp16 -> fp32 conversions, half the registers for x); always software-pipelined
-  {
-    uint4 xn[T], wn[R];
-#pragma unroll
-    for (int t = 0; t < T; t++) xn[t] = *reinterpret_cast<const uint4*>(x + xoff[t]);
-#pragma unroll
-    for (int r = 0; r < R; r++) wn[r] = ldg_nc16(W + woff[r]);
-    for (int g = 0; g < G; g++) {
-      const int gn = 256 * min(g + 1, G - 1);
-      uint4 xc[T];
-#pragma unroll
-      for (int t = 0; t < T; t++) {
-        xc[t] = xn[t];
-        xn[t] = *reinterpret_cast<const uint4*>(x + xoff[t] + gn);
-      }
-#pragma unroll
-      for (int r = 0; r < R; r++) {
-        const uint4 wc = wn[r];
-        wn[r] = ldg_nc16(W + woff[r] + gn);
-#pragma unroll
-        for (int t = 0; t < T; t++) acc[r * T + t] = dot8_packed(wc, xc[t], acc[r * T + t]);
-      }
-    }
-  }
-#else
   if constexpr (PIPE) {
     uint4 xr[T], wr[R];
 #pragma unroll
@@ -166,7 +140,6 @@ __global__ void __launch_bounds__(GEMM_WARPS * 32)
     }
   }
 
-#endif
   // accumulator index a = r*T + t ; after the transposing butterfly lane l holds accumulator 32*s + l
 #pragma unroll
   for (int s = 0; s < (R * T) / 32; s++) {
@@ -217,8 +190,8 @@ int launch_linear(const __half* W, const __half* bias, const __half* x, int ldx,
     set_error("ma_linear_f16: x/W must be 16-byte aligned and ldx a multiple of 8");
     return 1;
   }
-  // PIPE (254 registers, 2 CTAs/SM) wins while the grid is a few waves at most (B200, M = 16/64: fc2 -30 %, others
-  // +-5 %); at prefill sizes the 3-CTA/SM plain loop is 10 % faster (profiles/batched_kernels_r01.json)
+  // PIPE (254 registers, 2 CTAs/SM) for grids of a few waves at most (decode steps); the 3-CTA/SM plain loop for
+  // prefill sizes
   const bool pipe = M <= 512;
   if (seg == 64) {
     launch_seg<64>(W, bias, x, ldx, y, ldy, M, N, K, epi, st);

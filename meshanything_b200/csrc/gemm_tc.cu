@@ -1,30 +1,28 @@
-// gemm_tc.cu -- y = act(x W^T + b) on the 5th-generation tensor cores: tcgen05.mma with the accumulator in
-// TMEM, operands staged in shared memory by TMA (cp.async.bulk.tensor, 128-byte swizzle), mbarrier pipeline.
+// gemm_tc.cu -- y = act(x W^T + b) on the Hopper tensor cores: wgmma.mma_async with fp32 accumulators in registers,
+// operands staged in shared memory by TMA (cp.async.bulk.tensor, 128-byte swizzle), mbarrier pipeline.
 //
 // Used for the dense contractions of the stages that are compared under a tolerance (encoder a1-a8, detokenizer
 // a17-a18: SURVEY.md 2.2 G5/G6, ~200 GFLOP per shape).  The decoder keeps the canonical CUDA-core kernels: the
 // tensor core sums each K=16 slab in a hardware-defined order that a CPU oracle cannot restate bit for bit
 // (DESIGN.md section 3).
 //
-// One CTA = one 128x128 output tile, 192 threads:
-//   warp 0   TMA producer   (one elected lane): A tile [128 rows x 64 halfs], B tile [128 x 64] per stage, 4 stages
-//   warp 1   MMA issuer     (one elected lane): 4 x tcgen05.mma.cta_group::1.kind::f16 (M128 N128 K16) per stage,
-//                            tcgen05.commit -> frees the stage / signals the epilogue
-//   warps 2-5 epilogue      (TMEM lane quadrant = warp % 4): tcgen05.ld 32x32b.x32 -> + bias -> ReLU/GELU -> fp16 -> global
+// One CTA = one 128x128 output tile, 288 threads:
+//   warps 0-7  two consumer warpgroups: warpgroup g owns output rows m0 + 64g .. +63 and issues
+//              4 x wgmma m64n128k16 per stage (one wgmma group kept in flight; the stage before it is released)
+//   warp 8     TMA producer (one elected lane): A tile [128 rows x 64 halfs], B tile [128 x 64] per stage, 4 stages
 // Both operands are K-major ([rows][K] row-major), so D = A * B^T needs no transpose.  TMA zero-fills rows beyond M.
 #include "internal.h"
 #include "tc_common.cuh"
 
 namespace ma {
 
-constexpr int TC_BM = 128, TC_BN = 128, TC_BK = 64, TC_STAGES = 4, TC_THREADS = 192;
+constexpr int TC_BM = 128, TC_BN = 128, TC_BK = 64, TC_STAGES = 4, TC_THREADS = 288, TC_CONSUMER_WARPS = 8;
 constexpr uint32_t TC_STAGE_BYTES = (TC_BM + TC_BN) * TC_BK * 2;  // 32 KB
 
 struct alignas(1024) TcSmem {
   __half a[TC_STAGES][TC_BM * TC_BK];
   __half b[TC_STAGES][TC_BN * TC_BK];
-  uint64_t full[TC_STAGES], empty[TC_STAGES], tmem_full;
-  uint32_t tmem_base;
+  uint64_t full[TC_STAGES], empty[TC_STAGES];
 };
 
 __device__ __forceinline__ float gelu_erf_tc(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752440f)); }
@@ -38,30 +36,20 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
   const int m0 = blockIdx.y * TC_BM, n0 = blockIdx.x * TC_BN;
   const int nk = K / TC_BK;
 
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
+  if (threadIdx.x == 0) {
     for (int s = 0; s < TC_STAGES; s++) {
       mbar_init(&sm.full[s], 1);
-      mbar_init(&sm.empty[s], 1);
+      mbar_init(&sm.empty[s], TC_CONSUMER_WARPS);
     }
-    mbar_init(&sm.tmem_full, 1);
     mbar_fence_init();
   }
-  if (warp == 2) {  // TMEM: 128 fp32 columns x 128 lanes for the accumulator
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sm.tmem_base)),
-                 "n"(TC_BN)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = sm.tmem_base;
 
-  if (warp == 0) {
+  if (warp == TC_CONSUMER_WARPS) {
     // ---------------- TMA producer
     if (elect_one()) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b) : "memory");
       for (int kb = 0; kb < nk; kb++) {
         const int s = kb % TC_STAGES;
         const uint32_t ph = (kb / TC_STAGES) & 1;
@@ -71,60 +59,52 @@ __global__ void __launch_bounds__(TC_THREADS, 1)
         tma_load_2d(sm.b[s], &map_b, kb * TC_BK, n0, &sm.full[s]);
       }
     }
-  } else if (warp == 1) {
-    // ---------------- MMA issuer
-    // instruction descriptor: D=f32, A=B=f16, both K-major, N=128 (>>3 at bit 17), M=128 (>>4 at bit 24)
-    constexpr uint32_t idesc = (1u << 4) | (0u << 7) | (0u << 10) | ((TC_BN >> 3) << 17) | ((TC_BM >> 4) << 24);
-    for (int kb = 0; kb < nk; kb++) {
-      const int s = kb % TC_STAGES;
-      const uint32_t ph = (kb / TC_STAGES) & 1;
-      mbar_wait(&sm.full[s], ph);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t ad = umma_desc(sm.a[s]), bd = umma_desc(sm.b[s]);
-#pragma unroll
-        for (int k = 0; k < TC_BK / 16; k++)  // 32 bytes (16 halfs) further along K inside the 128-byte swizzle row
-          umma_f16(tmem, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), idesc, (kb | k) ? 1u : 0u);
-        umma_commit(&sm.empty[s]);                 // stage free once these MMAs have read it
-        if (kb == nk - 1) umma_commit(&sm.tmem_full);  // accumulator complete
-      }
-      __syncwarp();
-    }
-  } else {
-    // ---------------- epilogue: warp w reads TMEM lanes 32*(w%4) .. +31 = output rows m0 + 32*(w%4) + lane
-    const int q = warp & 3;
-    mbar_wait(&sm.tmem_full, 0);
-    tc_fence_after();
-    const int m = m0 + 32 * q + lane;
-#pragma unroll 1
-    for (int c0 = 0; c0 < TC_BN; c0 += 32) {
-      uint32_t r[32];
-      tmem_ld32(tmem + ((uint32_t)(32 * q) << 16) + (uint32_t)c0, r);
-      if (m < M) {
-        __half out[32];
-#pragma unroll
-        for (int j = 0; j < 32; j++) {
-          const int n = n0 + c0 + j;
-          float v = __uint_as_float(r[j]) + (bias ? __half2float(bias[n]) : 0.0f);
-          __half h = __float2half_rn(v);
-          if (epi == MA_EPI_RELU) {
-            if (__half2float(h) < 0.0f) h = __float2half_rn(0.0f);
-          } else if (epi == MA_EPI_GELU) {
-            h = __float2half_rn(gelu_erf_tc(__half2float(h)));
-          }
-          out[j] = h;
-        }
-        uint4* dst = reinterpret_cast<uint4*>(y + (long)m * ldy + n0 + c0);
-#pragma unroll
-        for (int j = 0; j < 4; j++) dst[j] = reinterpret_cast<const uint4*>(out)[j];
-      }
-    }
-    tc_fence_before();
+    return;
   }
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(TC_BN) : "memory");
+  // ---------------- consumers: warpgroup g = rows 64g .. 64g+63 of the tile
+  const int g = warp >> 2;
+  float acc[64];
+#pragma unroll
+  for (int i = 0; i < 64; i++) acc[i] = 0.0f;
+  for (int kb = 0; kb < nk; kb++) {
+    const int s = kb % TC_STAGES;
+    mbar_wait(&sm.full[s], (kb / TC_STAGES) & 1);
+    const uint64_t ad = gmma_desc(sm.a[s] + 64 * g * TC_BK), bd = gmma_desc(sm.b[s]);
+    wgmma_reg_fence<64>(acc);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < TC_BK / 16; k++)  // 32 bytes (16 halfs) further along K inside the 128-byte swizzle row
+      wgmma_ss<TC_BN>(acc, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), (kb | k) ? 1u : 0u);
+    wgmma_commit();
+    wgmma_reg_fence<64>(acc);
+    wgmma_wait<1>();                                        // the previous stage's wgmmas are complete
+    if (kb > 0 && lane == 0) mbar_arrive(&sm.empty[(kb - 1) % TC_STAGES]);
+  }
+  wgmma_wait<0>();
+  wgmma_reg_fence<64>(acc);
+  // ---------------- epilogue straight from the accumulator registers
+  const int r0 = m0 + 64 * g + 16 * (warp & 3) + (lane >> 2);
+#pragma unroll
+  for (int h = 0; h < 2; h++) {
+    const int m = r0 + 8 * h;
+    if (m >= M) continue;
+#pragma unroll
+    for (int i = 0; i < TC_BN / 8; i++) {
+      const int n = n0 + 8 * i + 2 * (lane & 3);
+      __half out[2];
+#pragma unroll
+      for (int e = 0; e < 2; e++) {
+        float v = acc[4 * i + 2 * h + e] + (bias ? __half2float(bias[n + e]) : 0.0f);
+        __half hv = __float2half_rn(v);
+        if (epi == MA_EPI_RELU) {
+          if (__half2float(hv) < 0.0f) hv = __float2half_rn(0.0f);
+        } else if (epi == MA_EPI_GELU) {
+          hv = __float2half_rn(gelu_erf_tc(__half2float(hv)));
+        }
+        out[e] = hv;
+      }
+      *reinterpret_cast<__half2*>(y + (long)m * ldy + n) = __halves2half2(out[0], out[1]);
+    }
   }
 }
 

@@ -1,12 +1,12 @@
-// gemm_ws.cu -- weight-streaming GEMM for FEW activation rows (M <= 128) on the 5th-generation tensor cores:
+// gemm_ws.cu -- weight-streaming GEMM for FEW activation rows (M <= 128) on the Hopper tensor cores:
 // y = act(x W^T + b) with the roles of the operands swapped ("swap-AB"): a 128-row block of the WEIGHT matrix is the
-// M = 128 operand of tcgen05.mma, the M <= 128 activation rows are its N operand (padded to 16 / 32 / 64 / 128), so a
-// decode step of a batch of sequences streams every weight exactly once through TMA at full tile efficiency instead
-// of spending 18-27 TFLOP/s of fp32 FMAs on it (profiles/batched_kernels_r01.json: 76 us per layer at M = 64).
+// M operand of wgmma (two warpgroups of 64 rows), the M <= 128 activation rows are its N operand (padded to
+// 16 / 32 / 64 / 128), so a decode step of a batch of sequences streams every weight exactly once through TMA at full
+// tile efficiency instead of spending fp32 FMAs on it.
 //
-// The decoder's matrices have only 8..65 row blocks, far fewer than the 148 SMs, so the K dimension is split across
-// CTAs as well (grid = row blocks x K slices ~ one CTA per SM).  Two ways to add the slices, both in slice order, so
-// the result never depends on timing:
+// The decoder's matrices have only 8..65 row blocks, fewer than the 132 SMs of an H100, so the K dimension is split
+// across CTAs as well (grid = row blocks x K slices ~ one CTA per SM).  Two ways to add the slices, both in slice
+// order, so the result never depends on timing:
 //   * cluster mode (default): the K slices of a row block are ONE thread-block cluster (2 / 4 / 8 CTAs).  Every CTA
 //     parks its fp32 tile in its own shared memory (the drained pipeline stages), the cluster synchronises, and CTA r
 //     finishes activation rows r, r + ks, ... by reading the ks tiles over distributed shared memory
@@ -19,9 +19,9 @@
 // each K = 16 slab in a hardware-defined order, so these results agree with the canonical kernels to fp32 rounding,
 // not bit for bit (DESIGN.md section 3).
 //
-// CTA = 192 threads: warp 0 TMA producer (W tile [128 x 64], x tile [MP x 64] per stage, 6-8 stages), warp 1 MMA issuer
-// (4 x tcgen05.mma.cta_group::1.kind::f16 M128 N=MP K16 per stage, accumulator [128 lanes x MP columns] in TMEM),
-// warps 2-5 epilogue (tcgen05.ld 32x32b: a thread owns one weight row = one output column n of y).
+// CTA = 288 threads: warps 0-7 two consumer warpgroups (warpgroup g: weight rows n0 + 64g .. +63, 4 x wgmma
+// m64 n=MP k16 per stage, accumulator [64 weight rows x MP activation rows] in registers), warp 8 TMA producer
+// (W tile [128 x 64], x tile [MP x 64] per stage, 6-8 stages).
 #include <stdlib.h>
 
 #include "internal.h"
@@ -29,8 +29,8 @@
 
 namespace ma {
 
-constexpr int WS_BN = 128, WS_BK = 64, WS_THREADS = 192;
-// pipeline depth: as many 16 KB weight tiles in flight as shared memory holds (a CTA streams at ~bytes in flight / 2 us)
+constexpr int WS_BN = 128, WS_BK = 64, WS_THREADS = 288, WS_CONSUMER_WARPS = 8;
+// pipeline depth: as many 16 KB weight tiles in flight as shared memory holds
 template <int MP> struct WsStages { static constexpr int value = MP <= 64 ? 8 : 6; };
 
 template <int MP>
@@ -38,14 +38,15 @@ struct alignas(1024) WsSmem {
   static constexpr int ST = WsStages<MP>::value;
   __half a[ST][WS_BN * WS_BK];
   __half b[ST][MP * WS_BK];
-  uint64_t full[ST], empty[ST], tmem_full;
-  uint32_t tmem_base;
+  uint64_t full[ST], empty[ST];
   int last;
 };
 
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
+// the 256 consumer threads only (the producer warp does not take part)
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 // 16 bytes from the shared memory of CTA `rank` of this cluster, at the same offset as `addr` in this CTA
 __device__ __forceinline__ float4 ld_dsmem_f4(uint32_t addr, uint32_t rank) {
   uint32_t ra;
@@ -75,42 +76,34 @@ __global__ void __launch_bounds__(WS_THREADS, 1)
                    float* __restrict__ part, unsigned* __restrict__ tickets, int npad, int cluster) {
   extern __shared__ __align__(1024) unsigned char smem_raw[];
   WsSmem<MP>& sm = *reinterpret_cast<WsSmem<MP>*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  constexpr int TCOLS = MP < 32 ? 32 : MP;   // TMEM allocations are powers of two >= 32 columns
   constexpr uint32_t STAGE_BYTES = (WS_BN + MP) * WS_BK * 2;
   constexpr int WS_STAGES = WsStages<MP>::value;
+  constexpr int NACC = MP / 2;   // accumulator registers per thread of an m64 nMP tile
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n0 = blockIdx.x * WS_BN;
   const int ks = gridDim.y, ky = blockIdx.y;
   const int kb0 = (int)(((long)nkb_total * ky) / ks), kb1 = (int)(((long)nkb_total * (ky + 1)) / ks);
   const int nk = kb1 - kb0;
+  // fp32 tile red[m][128] parked in the drained pipeline stages once every wgmma that read them has completed
+  float* red = reinterpret_cast<float*>(sm.a);
 
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
+  if (threadIdx.x == 0) {
     for (int s = 0; s < WS_STAGES; s++) {
       mbar_init(&sm.full[s], 1);
-      mbar_init(&sm.empty[s], 1);
+      mbar_init(&sm.empty[s], WS_CONSUMER_WARPS);
     }
-    mbar_init(&sm.tmem_full, 1);
     mbar_fence_init();
   }
-  if (warp == 2) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&sm.tmem_base)),
-                 "n"(TCOLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = sm.tmem_base;
 
   pdl_trigger();   // the next kernel may start its prologue (and, if it is a GEMM, its own weight tiles)
-  if (warp == 0) {
+  if (warp == WS_CONSUMER_WARPS) {
     // ---------------- TMA producer: this CTA's K slice of the weight row block (+ the matching columns of x).
     // The weights do not depend on the previous kernel: the first ring of weight tiles goes out BEFORE the grid
     // dependency resolves (programmatic dependent launch), the activation tiles after it.
     if (elect_one()) {
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_w) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(&map_x) : "memory");
       const int first = min(nk, WS_STAGES);
       for (int i = 0; i < first; i++) {
         mbar_expect_tx(&sm.full[i], STAGE_BYTES);
@@ -128,70 +121,68 @@ __global__ void __launch_bounds__(WS_THREADS, 1)
         tma_load_2d(sm.b[s], &map_x, (kb0 + i) * WS_BK, 0, &sm.full[s]);
       }
     }
-  } else if (warp == 1) {
-    // ---------------- MMA issuer: D[128 weight rows][MP activation rows] += Wtile * xtile^T
-    constexpr uint32_t idesc = (1u << 4) | (0u << 7) | (0u << 10) | ((uint32_t)(MP >> 3) << 17) | ((WS_BN >> 4) << 24);
+  } else {
+    // ---------------- consumers: D[64 weight rows][MP activation rows] += Wtile * xtile^T per warpgroup
+    const int g = warp >> 2, t = threadIdx.x;
+    float acc[NACC];
+#pragma unroll
+    for (int i = 0; i < NACC; i++) acc[i] = 0.0f;
     for (int i = 0; i < nk; i++) {
       const int s = i % WS_STAGES;
-      const uint32_t ph = (i / WS_STAGES) & 1;
-      mbar_wait(&sm.full[s], ph);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint64_t ad = umma_desc(sm.a[s]), bd = umma_desc(sm.b[s]);
+      mbar_wait(&sm.full[s], (i / WS_STAGES) & 1);
+      const uint64_t ad = gmma_desc(sm.a[s] + 64 * g * WS_BK), bd = gmma_desc(sm.b[s]);
+      wgmma_reg_fence<NACC>(acc);
+      wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < WS_BK / 16; k++) umma_f16(tmem, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), idesc, (i | k) ? 1u : 0u);
-        umma_commit(&sm.empty[s]);
-        if (i == nk - 1) umma_commit(&sm.tmem_full);
-      }
-      __syncwarp();
+      for (int k = 0; k < WS_BK / 16; k++) wgmma_ss<MP>(acc, ad + (uint64_t)(k * 2), bd + (uint64_t)(k * 2), (i | k) ? 1u : 0u);
+      wgmma_commit();
+      wgmma_reg_fence<NACC>(acc);
+      wgmma_wait<1>();
+      if (i > 0 && lane == 0) mbar_arrive(&sm.empty[(i - 1) % WS_STAGES]);
     }
-  } else {
-    // ---------------- epilogue: warp w reads TMEM lanes 32*(w%4).. = weight rows n0 + 32*(w%4) + lane
-    const int q = warp & 3;
-    const int et = 32 * q + lane;          // 0..127 inside the epilogue group
-    const int n = n0 + et;
-    mbar_wait(&sm.tmem_full, 0);
-    tc_fence_after();
-#pragma unroll 1
-    for (int c0 = 0; c0 < MP; c0 += 32) {
-      uint32_t r[32];
-      tmem_ld32(tmem + ((uint32_t)(32 * q) << 16) + (uint32_t)c0, r);
-      if (cluster) {
-        // park the tile as red[m][128] in the drained pipeline stages (every MMA that read them has completed)
-        float* red = reinterpret_cast<float*>(sm.a);
+    wgmma_wait<0>();
+    wgmma_reg_fence<NACC>(acc);
+    consumers_sync();   // every wgmma of both warpgroups has read its last stage: the stages may be overwritten
+    {
+      const int et = 64 * g + 16 * (warp & 3) + (lane >> 2);   // weight row inside the tile (+8 for h = 1)
 #pragma unroll
-        for (int j = 0; j < 32; j++) red[(c0 + j) * WS_BN + et] = __uint_as_float(r[j]);
-      } else if (n < N) {
+      for (int i = 0; i < MP / 8; i++)
 #pragma unroll
-        for (int j = 0; j < 32; j++) {
-          const int m = c0 + j;
-          if (m < M) {
-            if (ks == 1) y[(long)m * ldy + n] = ws_epilogue(__uint_as_float(r[j]), bias, n, epi);
-            else part[((long)ky * M + m) * npad + n] = __uint_as_float(r[j]);
-          }
+        for (int h = 0; h < 2; h++)
+#pragma unroll
+          for (int e = 0; e < 2; e++) red[(8 * i + 2 * (lane & 3) + e) * WS_BN + et + 8 * h] = acc[4 * i + 2 * h + e];
+    }
+    consumers_sync();
+    if (!cluster) {
+      const int et = t & (WS_BN - 1), n = n0 + et;
+      if (n < N) {
+        for (int m = t >> 7; m < M; m += 2) {
+          const float v = red[m * WS_BN + et];
+          if (ks == 1) y[(long)m * ldy + n] = ws_epilogue(v, bias, n, epi);
+          else part[((long)ky * M + m) * npad + n] = v;
         }
       }
     }
-    tc_fence_before();
     if (ks > 1 && !cluster) {
       // last CTA of this row block adds the K slices in slice order (deterministic) and finishes the rows
       __threadfence();
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (et == 0) {
+      consumers_sync();
+      if (t == 0) {
         const unsigned old = atomicAdd(&tickets[blockIdx.x], 1u);
         sm.last = (old == (unsigned)ks - 1u);
         if (sm.last) tickets[blockIdx.x] = 0u;   // ready for the next launch
       }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      if (sm.last) {
+      consumers_sync();
+      if (sm.last && t < 128) {
         // 128 threads = 32 column quads x 4 row groups; 4 rows x 4 K slices of float4 loads in flight per thread (one
-        // load at a time would serialise M * ks L2 round trips: 80 us measured).  Slices are added in slice order.
+        // load at a time would serialise M * ks L2 round trips).  Slices are added in slice order.
         __threadfence();
+        const int et = t;
         const int nq = n0 + 4 * (et & 31), mg = et >> 5;
         for (int m = mg; m < M; m += 16) {
-          float4 acc[4];
+          float4 acc4[4];
 #pragma unroll
-          for (int u = 0; u < 4; u++) acc[u] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
+          for (int u = 0; u < 4; u++) acc4[u] = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
 #pragma unroll 4
           for (int k = 0; k < ks; k++) {
 #pragma unroll
@@ -199,7 +190,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1)
               const int mm = m + 4 * u;
               if (mm < M) {
                 const float4 pv = __ldcg(reinterpret_cast<const float4*>(part + ((long)k * M + mm) * npad + nq));
-                acc[u].x += pv.x; acc[u].y += pv.y; acc[u].z += pv.z; acc[u].w += pv.w;
+                acc4[u].x += pv.x; acc4[u].y += pv.y; acc4[u].z += pv.z; acc4[u].w += pv.w;
               }
             }
           }
@@ -207,7 +198,7 @@ __global__ void __launch_bounds__(WS_THREADS, 1)
           for (int u = 0; u < 4; u++) {
             const int mm = m + 4 * u;
             if (mm < M) {
-              const float v4[4] = {acc[u].x, acc[u].y, acc[u].z, acc[u].w};
+              const float v4[4] = {acc4[u].x, acc4[u].y, acc4[u].z, acc4[u].w};
 #pragma unroll
               for (int i = 0; i < 4; i++)
                 if (nq + i < N) y[(long)mm * ldy + nq + i] = ws_epilogue(v4[i], bias, nq + i, epi);
@@ -222,14 +213,14 @@ __global__ void __launch_bounds__(WS_THREADS, 1)
     // done reading its peers' shared memory (no CTA may exit before that).
     __syncwarp();
     cluster_sync_all();
-    if (warp >= 2) {
+    if (warp < WS_CONSUMER_WARPS) {
       uint32_t rank;
       asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(rank));
-      const int et = 32 * (warp & 3) + lane;
-      const int nq = 4 * (et & 31), mg = et >> 5;      // 32 column quads x 4 row groups
+      const int et = threadIdx.x;
+      const int nq = 4 * (et & 31), mg = et >> 5;      // 32 column quads x 8 row groups
       const uint32_t red0 = smem_u32(sm.a);
-      // CTA `rank` finishes activation rows rank, rank + ks, ...; its 4 row groups take every 4th of those
-      for (int m = (int)rank + ks * mg; m < M; m += 4 * ks) {
+      // CTA `rank` finishes activation rows rank, rank + ks, ...; its 8 row groups take every 8th of those
+      for (int m = (int)rank + ks * mg; m < M; m += 8 * ks) {
         float4 acc = make_float4(0.0f, 0.0f, 0.0f, 0.0f);
         float4 pv[8];
 #pragma unroll
@@ -256,11 +247,6 @@ __global__ void __launch_bounds__(WS_THREADS, 1)
     }
     __syncwarp();
     cluster_sync_all();
-  }
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "n"(TCOLS) : "memory");
   }
 }
 
@@ -327,17 +313,18 @@ int launch_linear_ws(const __half* W, const __half* bias, const __half* x, int l
   const size_t avail = linear_ws_scratch_bytes() - WS_TICKETS * sizeof(unsigned);
   int ks, cluster = 0;
   if (g_ws_cluster) {
-    // cluster mode: the largest cluster of 8 / 4 / 2 K slices that keeps the grid within one wave of the SMs that can
-    // host such clusters on a B200 (1 CTA per SM: 15 x 8, 33 x 4, 74 x 2 co-resident, profiles/microbench_cluster_r02)
+    // cluster mode: the largest cluster of 8 / 4 / 2 K slices whose clusters are all resident at once.  On an H100
+    // (132 SMs) cudaOccupancyMaxActiveClusters gives 15 clusters of 8, 30 of 4 and 66 of 2 for this kernel at every MP
+    // (149-199 KB of shared memory, 1 CTA per SM): a cluster never straddles a GPC.
     ks = 1;
-    if (tiles * 8 <= 120 && nkb >= 16) ks = 8;          // out_proj, fc2: 8 row blocks -> 64 CTAs
-    else if (tiles * 4 <= 132 && nkb >= 8) ks = 4;      // qkv 24 -> 96, fc1 32 -> 128
-    else if (tiles * 2 <= 148 && nkb >= 4) ks = 2;      // lm_head 65 -> 130
+    if (tiles <= 15 && nkb >= 16) ks = 8;               // out_proj, fc2: 8 row blocks -> 64 CTAs
+    else if (tiles <= 30 && nkb >= 8) ks = 4;           // qkv 24 -> 96
+    else if (tiles <= 66 && nkb >= 4) ks = 2;           // fc1 32 -> 64, lm_head 65 -> 130
     cluster = ks > 1;
   } else {
-    // ticket mode: K is split only for matrices with few row blocks (out_proj, fc2: 8): the last-CTA fix-up costs ~1 us
-    // per K slice, more than a deep pipeline gains on 16+ CTAs (B200, M = 64: profiles/batched_kernels_r02.json)
-    ks = tiles >= 16 ? 1 : 148 / tiles;
+    // ticket mode: K is split only for matrices with few row blocks (out_proj, fc2: 8): the last-CTA fix-up costs about
+    // a microsecond per K slice, more than a deep pipeline gains on 16+ CTAs
+    ks = tiles >= 16 ? 1 : 132 / tiles;
     if (ks > 4) ks = 4;
     if (ks > nkb) ks = nkb;
     if (ks < 1) ks = 1;

@@ -34,8 +34,8 @@ bool check_launch(const char* what);
 int launch_linear(const __half* W, const __half* bias, const __half* x, int ldx, __half* y, int ldy, int M, int N,
                   int K, int epi, cudaStream_t st);
 
-// gemm_tc.cu (tcgen05 + TMA; tolerance-checked stages only)
-// attention_tc.cu (tcgen05 flash attention for the tolerance-compared stages)
+// gemm_tc.cu (wgmma + TMA; tolerance-checked stages only)
+// attention_tc.cu (wgmma flash attention for the tolerance-compared stages)
 bool attention_tc_supported(int ldq, int ldo, long T, long Tpad, int nkeys, const void* q, const void* K, const void* Vt,
                             const void* out);
 int launch_attention_tc(const __half* q, int ldq, const __half* K, const __half* Vt, long T, long Tpad, int H,
@@ -47,7 +47,7 @@ bool linear_tc_supported(int M, int N, int K, int ldx, int ldy, const void* x, c
 int launch_linear_tc(const __half* W, const __half* bias, const __half* x, int ldx, __half* y, int ldy, int M, int N,
                      int K, int epi, cudaStream_t st);
 
-// gemm_ws.cu (tcgen05 weight-streaming GEMM for M <= 128 rows: batched decode steps under a tolerance)
+// gemm_ws.cu (wgmma weight-streaming GEMM for M <= 128 rows: batched decode steps under a tolerance)
 size_t linear_ws_scratch_bytes();
 void linear_ws_set_mode(int cluster);
 int linear_ws_mode();   // 1: K slices reduced over distributed shared memory (default), 0: L2 + tickets
@@ -108,7 +108,7 @@ size_t mega_workspace_bytes();
 int mega_prepare(const ma_decoder_weights* w, void* mega_ws, cudaStream_t st);
 int mega_enqueue(const ma_decoder_weights* w, SeqState s, int tmax, __half* kv, void* mega_ws, const SampleArgs& sa,
                  int n_steps, int step_base, int trace, cudaStream_t st);
-int mega_supported();          // 1: 144 CTAs of the kernel's shape are co-resident on this device
+int mega_supported();          // 1: the kernel's row split fits this device's SM count and shared memory
 bool mega_fits(int tmax);
 void mega_set_debug(unsigned long long timeout_ns, int fault);
 int mega_error_flag_offset();

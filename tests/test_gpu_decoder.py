@@ -1,8 +1,8 @@
-"""-m gpu: ShapeOPT decoder generate() on the B200 against the CPU oracle (bit-exact ids AND fp16 logits)."""
+"""-m gpu: ShapeOPT decoder generate() on the GPU against the CPU oracle (bit-exact ids AND fp16 logits)."""
 import pytest
 import torch
 
-from tests.util import decoder_sd, random_prefix
+from tests.util import decoder_sd, random_prefix, skip_unless_persistent
 
 gpu = pytest.mark.gpu
 NL = 3          # layers of the small synthetic decoder used by most cases
@@ -35,6 +35,7 @@ def test_greedy_bit_exact_vs_oracle(small, flags):
     """free-running greedy decode: token ids and every step's fp16 logits equal the oracle's.
     flags: 0 persistent kernel, 16 per-phase kernels + PDL, 16|4 without PDL, |1 without CUDA graph, 2 batched kernels."""
     from meshanything_b200.decoder import Generator
+    skip_unless_persistent(flags)
     _, arena, oracle = small
     prefix = random_prefix(1, seed=3)
     gen = Generator(arena, 1, 257 + NEW)
@@ -58,6 +59,7 @@ def test_persistent_kernel_timeout_is_an_error(small):
     import time
     from meshanything_b200 import capi
     from meshanything_b200.decoder import Generator
+    skip_unless_persistent(0)
     _, arena, oracle = small
     prefix = random_prefix(1, seed=3)
     gen = Generator(arena, 1, 257 + NEW)
@@ -146,22 +148,34 @@ def test_eos_and_padding(small):
     assert int(lens1[0]) == len(ref_ids)
 
 
-@gpu
-def test_teacher_forced_logits(small):
-    """forced ids (incl. specials 0/1/2, which take the extra_embeds path) give the oracle's logits."""
+def _teacher_forced_logits(small, flags):
     from meshanything_b200.decoder import Generator
     _, arena, oracle = small
     prefix = random_prefix(1, seed=8)
     forced = [0, 5, 8194, 1, 2, 3, 77, 4000, 2, 9, 10, 11, 12]
     n = len(forced)
-    for flags in (0, 16, 2):
-        gen = Generator(arena, 1, 257 + n)
-        f = torch.tensor([forced], dtype=torch.int32)
-        ids, lens, logits = gen.generate(prefix.to(_dev()), n, forced_ids=f, want_logits=True, eos_id=-1, flags=flags)
-        _, ref_logits = oracle.generate(prefix[0], n, eos_id=-1, forced=forced, keep_logits=True)
-        assert ids[0].cpu().tolist() == forced
-        for i in range(n):
-            assert torch.equal(logits[i, 0].cpu().view(torch.int16), ref_logits[i].view(torch.int16)), (flags, i)
+    gen = Generator(arena, 1, 257 + n)
+    f = torch.tensor([forced], dtype=torch.int32)
+    ids, lens, logits = gen.generate(prefix.to(_dev()), n, forced_ids=f, want_logits=True, eos_id=-1, flags=flags)
+    _, ref_logits = oracle.generate(prefix[0], n, eos_id=-1, forced=forced, keep_logits=True)
+    assert ids[0].cpu().tolist() == forced
+    for i in range(n):
+        assert torch.equal(logits[i, 0].cpu().view(torch.int16), ref_logits[i].view(torch.int16)), (flags, i)
+
+
+@gpu
+def test_teacher_forced_logits(small):
+    """forced ids (incl. specials 0/1/2, which take the extra_embeds path) give the oracle's logits, on the per-phase
+    kernels (flags 16) and the batched kernels (flags 2)."""
+    for flags in (16, 2):
+        _teacher_forced_logits(small, flags)
+
+
+@gpu
+def test_teacher_forced_logits_persistent_kernel(small):
+    """the same on the persistent kernel (flags 0), where the device can host it."""
+    skip_unless_persistent(0)
+    _teacher_forced_logits(small, 0)
 
 
 @gpu
@@ -198,20 +212,30 @@ def test_tensor_core_decoder_logits_within_tolerance(small):
     print("tensor-core decoder: max |logit diff| vs oracle", worst)
 
 
-@gpu
-def test_long_context_crosses_chunks(small):
-    """600 new tokens: the context crosses three 256-key attention chunks (257 -> 857)."""
+def _long_context_crosses_chunks(small, flags):
     from meshanything_b200.decoder import Generator
     _, arena, oracle = small
     prefix = random_prefix(1, seed=13)
     n = 600
     ref_ids, _ = oracle.generate(prefix[0], n)
-    for flags in (0, 16):
-        gen = Generator(arena, 1, 257 + n)
-        ids, _ = gen.generate(prefix.to(_dev()), n, flags=flags)
-        assert ids[0].cpu().tolist() == ref_ids, flags
-        if flags == 0:
-            assert gen.mega_error() == 0
+    gen = Generator(arena, 1, 257 + n)
+    ids, _ = gen.generate(prefix.to(_dev()), n, flags=flags)
+    assert ids[0].cpu().tolist() == ref_ids, flags
+    if flags == 0:
+        assert gen.mega_error() == 0
+
+
+@gpu
+def test_long_context_crosses_chunks(small):
+    """600 new tokens: the context crosses three 256-key attention chunks (257 -> 857); per-phase kernels."""
+    _long_context_crosses_chunks(small, 16)
+
+
+@gpu
+def test_long_context_crosses_chunks_persistent_kernel(small):
+    """the same on the persistent kernel, where the device can host it."""
+    skip_unless_persistent(0)
+    _long_context_crosses_chunks(small, 0)
 
 
 @gpu
@@ -255,12 +279,7 @@ def test_full_depth_config1_golden():
         assert got == ref
 
 
-@gpu
-@pytest.mark.slow
-def test_full_depth_config2_golden():
-    """BASELINE.json configs[1] parity: 24 layers, 800-face cap (7202 new tokens, contexts up to 7458), batch 1, greedy.
-    The free-running token ids equal the CPU oracle's (tests/golden/decoder_greedy_seed0_F800.json, generated by
-    tests/golden/make_golden.py greedy800), for the persistent kernel and for the per-phase kernels."""
+def _full_depth_config2_golden(flags):
     import json, os
     from meshanything_b200.decoder import DecoderArena, Generator
     gold = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "decoder_greedy_seed0_F800.json")))["ids"]
@@ -268,23 +287,33 @@ def test_full_depth_config2_golden():
     prefix = random_prefix(1, seed=1).to(_dev())
     n = 800 * 9 + 2
     gen = Generator(arena, 1, 257 + n)
-    for flags in (0, 16):
-        ids, lens = gen.generate(prefix, n, flags=flags)
-        got = ids[0].cpu().tolist()
-        first_bad = next((i for i, (a, b) in enumerate(zip(got, gold)) if a != b), None)
-        assert first_bad is None, f"flags={flags}: first divergence at step {first_bad}"
-        assert int(lens[0]) == n
-    assert gen.mega_error() == 0
+    ids, lens = gen.generate(prefix, n, flags=flags)
+    got = ids[0].cpu().tolist()
+    first_bad = next((i for i, (a, b) in enumerate(zip(got, gold)) if a != b), None)
+    assert first_bad is None, f"flags={flags}: first divergence at step {first_bad}"
+    assert int(lens[0]) == n
+    if flags == 0:
+        assert gen.mega_error() == 0
 
 
 @gpu
 @pytest.mark.slow
-def test_long_context_config5_golden():
-    """BASELINE.json configs[4] length (V1 architecture, 1600-face cap: 14402 new tokens, contexts up to 14658 = 58
-    attention chunks, four rounds of attention items in the persistent kernel).  First 4 layers of the synthetic
-    decoder; ids equal the CPU oracle's (tests/golden/decoder_greedy_seed0_F1600.json, make_golden.py greedy1600)
-    for the persistent kernel, the per-phase kernels, and a batch of 2 on the batched kernels (row 0 = the golden
-    prefix, row 1 another prefix: rows are independent)."""
+def test_full_depth_config2_golden():
+    """BASELINE.json configs[1] parity: 24 layers, 800-face cap (7202 new tokens, contexts up to 7458), batch 1, greedy.
+    The free-running token ids on the per-phase kernels equal the CPU oracle's (tests/golden/decoder_greedy_seed0_F800.json,
+    generated by tests/golden/make_golden.py greedy800)."""
+    _full_depth_config2_golden(16)
+
+
+@gpu
+@pytest.mark.slow
+def test_full_depth_config2_golden_persistent_kernel():
+    """the same on the persistent kernel, where the device can host it."""
+    skip_unless_persistent(0)
+    _full_depth_config2_golden(0)
+
+
+def _long_context_config5_golden(flags, batched):
     import json, os
     from meshanything_b200.decoder import DecoderArena, Generator
     g = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "decoder_greedy_seed0_F1600.json")))
@@ -294,18 +323,36 @@ def test_long_context_config5_golden():
     prefix = random_prefix(1, seed=1).to(_dev())
     n = 1600 * 9 + 2
     gen = Generator(arena, 1, 257 + n)
-    for flags in (0, 16):
-        ids, lens = gen.generate(prefix, n, flags=flags, eos_id=eos)
-        got = ids[0].cpu().tolist()
-        first_bad = next((i for i, (a, b) in enumerate(zip(got, gold)) if a != b), None)
-        assert first_bad is None, f"flags={flags}: first divergence at step {first_bad}"
-        assert int(lens[0]) == n
-        if flags == 0:
-            assert gen.mega_error() == 0
-    two = torch.cat([prefix, random_prefix(1, seed=5).to(_dev())], dim=0)
-    gen2 = Generator(arena, 2, 257 + n)
-    ids2, _ = gen2.generate(two, n, eos_id=eos)
-    assert ids2[0].cpu().tolist() == gold
+    ids, lens = gen.generate(prefix, n, flags=flags, eos_id=eos)
+    got = ids[0].cpu().tolist()
+    first_bad = next((i for i, (a, b) in enumerate(zip(got, gold)) if a != b), None)
+    assert first_bad is None, f"flags={flags}: first divergence at step {first_bad}"
+    assert int(lens[0]) == n
+    if flags == 0:
+        assert gen.mega_error() == 0
+    if batched:
+        two = torch.cat([prefix, random_prefix(1, seed=5).to(_dev())], dim=0)
+        gen2 = Generator(arena, 2, 257 + n)
+        ids2, _ = gen2.generate(two, n, eos_id=eos)
+        assert ids2[0].cpu().tolist() == gold
+
+
+@gpu
+@pytest.mark.slow
+def test_long_context_config5_golden():
+    """BASELINE.json configs[4] length (V1 architecture, 1600-face cap: 14402 new tokens, contexts up to 14658 = 58
+    attention chunks).  First 4 layers of the synthetic decoder; ids equal the CPU oracle's
+    (tests/golden/decoder_greedy_seed0_F1600.json, make_golden.py greedy1600) for the per-phase kernels and for a batch
+    of 2 on the batched kernels (row 0 = the golden prefix, row 1 another prefix: rows are independent)."""
+    _long_context_config5_golden(16, batched=True)
+
+
+@gpu
+@pytest.mark.slow
+def test_long_context_config5_golden_persistent_kernel():
+    """the same length on the persistent kernel (four rounds of attention items), where the device can host it."""
+    skip_unless_persistent(0)
+    _long_context_config5_golden(0, batched=False)
 
 
 @gpu

@@ -151,7 +151,7 @@ def test_attention_decode_stream_bit_exact(T, nk):
 @pytest.mark.parametrize("M,N,K,epi", [(128, 128, 256, 0), (257, 768, 768, 0), (4096, 1536, 768, 0), (130, 128, 256, 1),
                                         (1057, 3072, 768, 2), (300, 768, 3072, 0), (64, 1152, 768, 0)])
 def test_linear_tensor_core(M, N, K, epi):
-    """tcgen05/TMA GEMM (encoder / detokenizer): fp16 in, fp32 accumulate in the hardware's order -> compared with an
+    """wgmma/TMA GEMM (encoder / detokenizer): fp16 in, fp32 accumulate in the hardware's order -> compared with an
     fp64 product rounded once to fp16 (tolerance: one fp16 ulp + fp32 accumulation noise) and with the canonical kernel."""
     from meshanything_b200 import capi
     g = torch.Generator().manual_seed(M + N + K)
@@ -180,7 +180,7 @@ def test_linear_tensor_core(M, N, K, epi):
                                         (2, 200, 64, 0)])
 @pytest.mark.parametrize("cluster", [1, 0])
 def test_linear_weight_streaming_tensor_core(M, N, K, epi, cluster):
-    """gemm_ws_kernel (swap-AB tcgen05 GEMM for M <= 128 rows, K split across CTAs): K slices added over distributed
+    """gemm_ws_kernel (swap-AB wgmma GEMM for M <= 128 rows, K split across CTAs): K slices added over distributed
     shared memory inside a thread-block cluster (cluster = 1, the default) or through L2 with an atomic ticket
     (cluster = 0).  fp16 in, fp32 accumulate in the hardware's order -> compared with an fp64 product rounded once to
     fp16 and with the canonical kernel; two runs give identical bits (the K-slice sum is taken in slice order)."""
@@ -306,9 +306,9 @@ def test_sampler_draw_frequencies():
 @pytest.mark.parametrize("S,rows,n,H", [(2, 257, 4096, 12), (3, 257, 257, 12), (2, 256, 256, 12), (1, 311, 311, 12),
                                         (1, 128, 128, 2), (1, 5, 70, 1)])
 def test_attention_tc_vs_fp64(S, rows, n, H):
-    """tcgen05 flash attention (ma_attention_tc_f16) against softmax attention in float64 on the same fp16 inputs.
+    """wgmma flash attention (ma_attention_tc_f16) against softmax attention in float64 on the same fp16 inputs.
     Stated tolerance: 2e-3 absolute on outputs of magnitude <= ~1 (P is rounded to fp16 before P.V, as in the canonical
-    kernel; accumulation is fp32 in TMEM).  Also checks the V^T layout kernel bit for bit."""
+    kernel; accumulation is fp32 in registers).  Also checks the V^T layout kernel bit for bit."""
     from meshanything_b200 import capi
     g = torch.Generator().manual_seed(S * 1000 + n)
     q = (torch.randn(S * rows, H * 64, generator=g) * 1.0).half()

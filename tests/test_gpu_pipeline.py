@@ -1,4 +1,4 @@
-"""-m gpu: encoder (a1-a8), detokenizer (a17-a18) and the MeshAnything.forward drop-in on the B200.
+"""-m gpu: encoder (a1-a8), detokenizer (a17-a18) and the MeshAnything.forward drop-in on the GPU.
 
 Floating-point stages are compared with the fp32 torch restatement (oracle/torch_ref.py, itself pinned to the
 reference's own modules) under a stated tolerance: the GPU path rounds every Linear input/output to fp16 as CUDA
@@ -15,7 +15,7 @@ from meshanything_b200.inputs import synthetic_pc_normal
 
 gpu = pytest.mark.gpu
 
-# stated tolerances (measured margins in DESIGN.md section 6)
+# stated tolerances (DESIGN.md section 6)
 TOL_PF_MAX, TOL_PF_MEAN = 1.5e-2, 2.5e-3      # measured 3.5e-3 / 5.9e-4 (unit-variance LayerNorm output after 9 blocks)
 TOL_PREFIX_MAX, TOL_PREFIX_MEAN = 4e-2, 6e-3  # measured 1.0e-2 / 1.6e-3 (std 1.4, 16 more fp16-stream blocks + cond_proj)
 F_SMALL = 8
@@ -51,7 +51,7 @@ def test_encoder_vs_fp32_reference(full):
 
 @gpu
 def test_encoder_and_detokenizer_with_tensor_core_attention(full):
-    """ma_set_tensor_cores(2): attention of the encoder / detokenizer on tcgen05 too -- same stated tolerances against
+    """ma_set_tensor_cores(2): attention of the encoder / detokenizer on the tensor cores too -- same stated tolerances against
     the fp32 restatement, and close to the default (canonical attention) path."""
     from meshanything_b200 import capi
     from meshanything_b200.encoder import EncoderArena, TokenizerArena
@@ -182,8 +182,6 @@ def test_forward_drop_in(full):
           "agreement %.3f; teacher-forced logits max |diff| %.4f mean %.5f, argmax agreement %.4f (%d positions with margin > 0.25)"
           % (first_div, len(ref_ids), agree, float(d.max()), float(d.mean()),
              float((gl.argmax(1) == rl.argmax(1)).float().mean()), int(clear.sum())))
-    # measured on the B200 (round 2): first divergence at step 95 of 578, free-running agreement 0.972; teacher-forced
-    # max |diff| 7.8e-3, mean 1.1e-3, argmax agreement 0.995 (the 3 disagreeing positions have margins below 0.01)
     assert first_div >= 1
     assert d.max() < 5e-2 and d.mean() < 5e-3
     assert torch.equal(gl.argmax(1)[clear], rl.argmax(1)[clear])
@@ -259,7 +257,7 @@ def test_main_cli_continuous_batching(tmp_path):
 
 @gpu
 def test_kernel_selections_all_meet_the_tolerance(full):
-    """ma_set_tensor_cores 0 (canonical CUDA-core kernels), 1 (tcgen05 GEMMs, canonical attention) and 2 (default):
+    """ma_set_tensor_cores 0 (canonical CUDA-core kernels), 1 (wgmma GEMMs, canonical attention) and 2 (default):
     every selection stays inside the stated encoder tolerance, and they agree with each other to fp16 noise."""
     from meshanything_b200 import capi
     from meshanything_b200.encoder import EncoderArena

@@ -4,9 +4,9 @@
 
 Times, with CUDA events on the launching stream (20 launches after 5 warm-ups, inputs larger than L2 or rotated):
   * attention_kernel (ma_attention_f16) for B rows x 16 heads at several context lengths -> achieved KV GB/s;
-  * the canonical fp32-FMA GEMM (ma_linear_f16), the tiled tcgen05 GEMM (ma_linear_tc_f16) and the weight-streaming
-    tcgen05 GEMM (ma_linear_ws_f16) at M = B for the five decoder shapes -> us per call, weight GB/s, TFLOP/s.
-Prints one JSON object (committed under profiles/ by hand)."""
+  * the canonical fp32-FMA GEMM (ma_linear_f16), the tiled wgmma GEMM (ma_linear_tc_f16) and the weight-streaming
+    wgmma GEMM (ma_linear_ws_f16) at M = B for the five decoder shapes -> us per call, weight GB/s, TFLOP/s.
+Prints one JSON object."""
 import argparse
 import ctypes as C
 import json
@@ -89,9 +89,9 @@ def main():
                     f(w, b, x)
             return g
         rec = {"name": name, "N": N, "K": K}
-        for tag, f in (("canon", capi.linear_f16), ("tcgen05", capi.linear_tc_f16), ("tcgen05_ws", capi.linear_ws_f16),
-                       ("tcgen05_ws_ticket", capi.linear_ws_f16)):
-            L.ma_linear_ws_set_mode(0 if tag == "tcgen05_ws_ticket" else 1)
+        for tag, f in (("canon", capi.linear_f16), ("wgmma", capi.linear_tc_f16), ("wgmma_ws", capi.linear_ws_f16),
+                       ("wgmma_ws_ticket", capi.linear_ws_f16)):
+            L.ma_linear_ws_set_mode(0 if tag == "wgmma_ws_ticket" else 1)
             try:
                 g = graph_of(f)
                 us = timed(g.replay, n=10, warm=2) / 24

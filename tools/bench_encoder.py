@@ -1,5 +1,5 @@
 """Encoder / detokenizer stage timings under the three kernel selections of ma_set_tensor_cores (0: canonical CUDA-core
-kernels, 1: tcgen05 GEMMs, 2: tcgen05 GEMMs + tcgen05 attention).  CUDA events, 5 timed runs after 2 warm-ups.
+kernels, 1: wgmma GEMMs, 2: wgmma GEMMs + wgmma attention).  CUDA events, 5 timed runs after 2 warm-ups.
 
     python tools/bench_encoder.py [--batch 8] [--faces 800]
 """
