@@ -284,6 +284,26 @@ size_t ma_sample_surface_workspace_bytes(int n_faces);
 int ma_sample_surface(const float* vertices, const int32_t* faces, int n_faces, int n_samples, unsigned long long seed,
                       void* out_pc_normal, int32_t* out_face_idx, void* ws, void* stream);
 
+/* ---- watertight remesh of `--mc` (mesh2sdf.core.compute + skimage.measure.marching_cubes of
+ * /root/reference/mesh_to_pc.py:13-40; csrc/watertight.cu) ----------------------------------------------------------
+ * Narrow-band unsigned distance field: out_field fp32 [n][n][n], out_field[i][j][k] = min(band, Euclidean distance from
+ * the grid point (-1 + i dx, -1 + j dx, -1 + k dx), dx = 2/n, to the nearest face).  vertices fp32 [V][3], faces int32
+ * [F][3] (indices in range: the caller checks them); degenerate faces count as their segments or point.  One fixed fp32
+ * formula and an order-independent minimum: bit-deterministic.  2 <= n <= 1024, band > 0. */
+int ma_udf_grid(const float* vertices, const int32_t* faces, int n_faces, int n, float band, float* out_field,
+                void* stream);
+/* Marching cubes of field fp32 [n][n][n] at `level` (a corner is inside when f < level) over the (n-1)^3 cells.
+ * ws: ma_marching_cubes_workspace_bytes(n) bytes (needs the device: it sizes CUB's scan).  ma_marching_cubes_count
+ * classifies the cells, scans the counts and writes {vertices, triangles} to counts_host (int64 [2], host memory); it
+ * synchronises the stream.  ma_marching_cubes_emit then writes out_vertices fp32 [V][3] (index space: a + t (b - a)
+ * along the crossed grid edge, t = (level - f_a) / (f_b - f_a)) and out_faces int32 [T][3], from the same ws and field.
+ * One vertex per crossed edge, ordered by lower grid point then x, y, z edge; triangles by cell then table order; the
+ * right-hand normal of every triangle points toward increasing field. */
+size_t ma_marching_cubes_workspace_bytes(int n);
+int ma_marching_cubes_count(const float* field, int n, float level, void* ws, int64_t* counts_host, void* stream);
+int ma_marching_cubes_emit(const float* field, int n, float level, const void* ws, float* out_vertices,
+                           int32_t* out_faces, void* stream);
+
 /* number of kernels launched by the library since load (bench.py's gpu_launches) */
 unsigned long long ma_launch_count(void);
 

@@ -1,9 +1,10 @@
 """Drop-in for /root/reference/mesh_to_pc.py: mesh -> (4096, 6) fp16 point cloud with normals.
 
-Uses trimesh / mesh2sdf / skimage when they are installed (same calls as the reference); otherwise a
-small numpy implementation of area-weighted surface sampling (what `trimesh.Trimesh.sample` does) is
-used (OBJ and ASCII/binary PLY readers included) and `marching_cubes=True` raises (mesh2sdf is required for the
-watertight conversion).
+On a GPU box with the library, surface sampling (csrc/surface.cu) and the watertight remesh of `marching_cubes=True`
+(distance field + marching cubes, csrc/watertight.cu) run in CUDA.  Otherwise, or with MA_PC_SAMPLER=host, trimesh /
+mesh2sdf / skimage are used when they are installed (same calls as the reference); without them a small numpy
+implementation of area-weighted surface sampling (what `trimesh.Trimesh.sample` does) is used (OBJ and ASCII/binary
+PLY readers included) and `marching_cubes=True` raises (mesh2sdf is required for the host-side watertight conversion).
 """
 import numpy as np
 
@@ -147,8 +148,13 @@ def normalize_vertices(vertices, scale=0.9):
 
 
 def export_to_watertight(normalized_mesh, octree_depth: int = 7):
-    """Watertight remesh used by `--mc` (reference mesh_to_pc.py:13-40): unsigned distance field on a 2^depth grid
-    (mesh2sdf), marching cubes at iso level 2/size, mapped back to the input frame."""
+    """Watertight remesh used by `--mc` (reference mesh_to_pc.py:13-40): unsigned distance field on a 2^depth grid,
+    marching cubes at iso level 2/size, mapped back to the input frame.  On a GPU box both stages run in CUDA
+    (ma_udf_grid + ma_marching_cubes_*, csrc/watertight.cu); otherwise, or with MA_PC_SAMPLER=host, mesh2sdf and
+    scikit-image do it as in the reference."""
+    gpu = _gpu_sampler()
+    if gpu is not None:
+        return _watertight_gpu(normalized_mesh, octree_depth, *gpu)
     try:
         import mesh2sdf.core
         import skimage.measure
@@ -160,6 +166,23 @@ def export_to_watertight(normalized_mesh, octree_depth: int = 7):
     verts, faces, normals, _ = skimage.measure.marching_cubes(field, 2 / size)
     verts = (verts / size * 2 - 1) / factor + centre
     return trimesh.Trimesh(verts, faces, normals=normals)
+
+
+def _watertight_gpu(mesh, octree_depth, capi, torch):
+    """Normalise in float64 on the host, narrow-band distance field (band 3 dx) and marching cubes at level dx = 2/size
+    on the GPU, vertices mapped back with (v / size * 2 - 1) / factor + centre."""
+    size = 2 ** octree_depth
+    unit_vertices, centre, factor = normalize_vertices(np.asarray(mesh.vertices, dtype=np.float64))
+    dev = torch.device("cuda", torch.cuda.current_device())
+    v = torch.as_tensor(unit_vertices.astype(np.float32), device=dev)
+    f = torch.as_tensor(np.asarray(mesh.faces, dtype=np.int32), device=dev)
+    field = capi.udf_grid(v, f, size)
+    verts, faces = capi.marching_cubes(field, 2.0 / size)
+    verts = (verts.cpu().numpy().astype(np.float64) / size * 2 - 1) / factor + centre
+    faces = faces.cpu().numpy().astype(np.int64)
+    if trimesh is not None:
+        return trimesh.Trimesh(verts, faces)
+    return SimpleMesh(verts, faces)
 
 
 def _gpu_sampler():

@@ -45,6 +45,7 @@ EXPORTS = [
     "ma_decode_slots_init", "ma_decode_slot_prefill", "ma_decode_slots_step", "ma_decode_slots_poll",
     "ma_mega_set_debug", "ma_linear_ws_set_mode", "ma_decode_slots_seek", "ma_decode_slot_stream", "ma_linear_ws_scratch_bytes", "ma_linear_ws_f16",
     "ma_sample_surface_workspace_bytes", "ma_sample_surface", "ma_tensor_core_linear_counts", "ma_decode_persistent_supported",
+    "ma_udf_grid", "ma_marching_cubes_workspace_bytes", "ma_marching_cubes_count", "ma_marching_cubes_emit",
 ]
 
 
@@ -113,6 +114,11 @@ def lib():
     L.ma_sample_surface_workspace_bytes.argtypes = [C.c_int]
     L.ma_sample_surface_workspace_bytes.restype = C.c_size_t
     L.ma_sample_surface.argtypes = [_vp, _vp, C.c_int, C.c_int, C.c_ulonglong, _vp, _vp, _vp, _vp]
+    L.ma_udf_grid.argtypes = [_vp, _vp, C.c_int, C.c_int, C.c_float, _vp, _vp]
+    L.ma_marching_cubes_workspace_bytes.argtypes = [C.c_int]
+    L.ma_marching_cubes_workspace_bytes.restype = C.c_size_t
+    L.ma_marching_cubes_count.argtypes = [_vp, C.c_int, C.c_float, _vp, C.POINTER(C.c_int64), _vp]
+    L.ma_marching_cubes_emit.argtypes = [_vp, C.c_int, C.c_float, _vp, _vp, _vp, _vp]
     L.ma_linear_tc_f16.argtypes = [_vp, _vp, _vp, C.c_int, _vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _vp]
     L.ma_set_tensor_cores.argtypes = [C.c_int]
     L.ma_tensor_core_linear_counts.argtypes = [C.POINTER(C.c_ulonglong), C.POINTER(C.c_ulonglong)]
@@ -172,6 +178,45 @@ def sample_surface(vertices: torch.Tensor, faces: torch.Tensor, n_samples: int, 
     check(lib().ma_sample_surface(ptr(v), ptr(f), F, n_samples, int(seed), ptr(out), ptr(idx), ptr(ws), stream_ptr()),
           "ma_sample_surface")
     return (out, idx) if want_index else out
+
+
+def udf_grid(vertices: torch.Tensor, faces: torch.Tensor, n: int, band: Optional[float] = None) -> torch.Tensor:
+    """Narrow-band unsigned distance field fp32 [n, n, n]: field[i, j, k] = min(band, distance from the grid point
+    (-1 + i dx, -1 + j dx, -1 + k dx), dx = 2/n, to the nearest face); band defaults to 3 dx."""
+    _need_cuda(vertices, faces)
+    v = vertices.to(torch.float32).contiguous()
+    f = faces.to(torch.int32).contiguous()
+    if v.dim() != 2 or v.shape[1] != 3 or f.dim() != 2 or f.shape[1] != 3:
+        raise ValueError("udf_grid: vertices [V, 3] and faces [F, 3]")
+    if not bool(torch.isfinite(v).all()):
+        raise ValueError("udf_grid: non-finite vertex coordinates")
+    if f.numel() and (int(f.min()) < 0 or int(f.max()) >= v.shape[0]):
+        raise ValueError(f"udf_grid: face indices outside [0, {v.shape[0]})")
+    if not 2 <= n <= 1024:
+        raise ValueError("udf_grid: 2 <= n <= 1024")
+    band = 3.0 * 2.0 / n if band is None else float(band)
+    out = torch.empty((n, n, n), dtype=torch.float32, device=v.device)
+    check(lib().ma_udf_grid(ptr(v), ptr(f), f.shape[0], n, C.c_float(band), ptr(out), stream_ptr()), "ma_udf_grid")
+    return out
+
+
+def marching_cubes(field: torch.Tensor, level: float):
+    """Marching cubes of fp32 [n, n, n] at `level` -> (vertices fp32 [V, 3] in index space, faces int32 [T, 3]); the
+    faces' right-hand normals point toward increasing field.  Reads the two counts back once (synchronises)."""
+    _need_cuda(field)
+    fld = field.to(torch.float32).contiguous()
+    n = fld.shape[0]
+    if fld.dim() != 3 or fld.shape != (n, n, n) or not 2 <= n <= 1024:
+        raise ValueError("marching_cubes: field [n, n, n], 2 <= n <= 1024")
+    ws = torch.empty(lib().ma_marching_cubes_workspace_bytes(n), dtype=torch.uint8, device=fld.device)
+    counts = (C.c_int64 * 2)()
+    check(lib().ma_marching_cubes_count(ptr(fld), n, C.c_float(level), ptr(ws), counts, stream_ptr()),
+          "ma_marching_cubes_count")
+    verts = torch.empty((counts[0], 3), dtype=torch.float32, device=fld.device)
+    tris = torch.empty((counts[1], 3), dtype=torch.int32, device=fld.device)
+    check(lib().ma_marching_cubes_emit(ptr(fld), n, C.c_float(level), ptr(ws), ptr(verts), ptr(tris), stream_ptr()),
+          "ma_marching_cubes_emit")
+    return verts, tris
 
 
 def tensor_core_linear_counts():
