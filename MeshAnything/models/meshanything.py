@@ -11,7 +11,7 @@ There is no PyTorch / CPU fallback: without a CUDA device or without the shared 
 """
 from __future__ import annotations
 
-from typing import Dict
+from typing import Dict, NamedTuple
 
 import torch
 from torch import nn
@@ -19,6 +19,15 @@ from torch import nn
 from MeshAnything.miche.encode import load_model
 from meshanything_b200 import checkpoint as _ck
 from meshanything_b200.config import DEC
+
+
+class Candidates(NamedTuple):
+    """What MeshAnything.forward_candidates returns."""
+    best: torch.Tensor                # [B, F, 3, 3] the kept candidate of every shape
+    meshes: torch.Tensor              # [B, N, F, 3, 3] every candidate
+    chamfer: torch.Tensor             # [B, N] fp64, lower is better (+inf: no face with an area)
+    normal_consistency: torch.Tensor  # [B, N] fp64 in [0, 1]
+    index: torch.Tensor               # [B] int64, the kept candidate
 
 
 class MeshAnything(nn.Module):
@@ -104,6 +113,33 @@ class MeshAnything(nn.Module):
         out = self._tok.detokenize(ids, point_feature, self.n_max_triangles)
         gen.check()   # a timed-out hand-off inside the persistent decode kernel is an error, never a wrong mesh
         return out
+
+    # ------------------------------------------------------------------ best of N samples
+    @torch.no_grad()
+    def forward_candidates(self, pc_normal, num_samples: int) -> Candidates:
+        """Not in the reference (whose app tells users to re-roll the seed when a result is unsatisfying): samples
+        `num_samples` meshes of every shape as one batch and keeps the one closest to the input cloud.
+
+        One sampled `forward` of pc_normal.repeat_interleave(num_samples, 0) -- candidate k of shape b is row
+        b * num_samples + k of that call, bit for bit, and draws from its Philox stream -- then `metrics.score` against
+        the shape's cloud and the lowest chamfer (lowest index on ties).  Returns Candidates(best [B, F, 3, 3],
+        meshes [B, N, F, 3, 3], chamfer [B, N], normal_consistency [B, N], index [B])."""
+        from meshanything_b200 import metrics
+        n = int(num_samples)
+        if n < 1:
+            raise ValueError(f"num_samples must be >= 1, got {num_samples}")
+        if self._dec is None:
+            raise RuntimeError("MeshAnything has no weights: call load_state_dict first")
+        pc = torch.as_tensor(pc_normal)
+        if not pc.is_cuda:
+            pc = pc.to(self._device)
+        B = pc.shape[0]
+        out = self.forward(pc.repeat_interleave(n, 0), sampling=True)
+        meshes = out.reshape(B, n, *out.shape[1:])
+        s = metrics.score(meshes, pc)
+        index = metrics.select(s["chamfer"])
+        best = meshes[torch.arange(B, device=meshes.device), index]
+        return Candidates(best, meshes, s["chamfer"], s["normal_consistency"], index)
 
     # ------------------------------------------------------------------ queue of shapes (continuous batching)
     @torch.no_grad()

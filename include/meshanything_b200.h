@@ -304,6 +304,24 @@ int ma_marching_cubes_count(const float* field, int n, float level, void* ws, in
 int ma_marching_cubes_emit(const float* field, int n, float level, const void* ws, float* out_vertices,
                            int32_t* out_faces, void* stream);
 
+/* ---- scoring of generated meshes against their input cloud (best-of-N sampling; csrc/mesh_score.cu) -------------
+ * S shapes x N candidates.  meshes fp32 [S][N][F][3][3] face soups in the output frame (a face is valid iff its first
+ * coordinate is not NaN; valid faces must be finite); clouds fp32 [S][P][6] (xyz | normal), finite, already mapped to
+ * the output frame.  out fp64 [S][N][4] = {p2m, m2p, nc_p, nc_m} as DESIGN.md section 1 (f6) defines them:
+ *   p2m   mean over the cloud points of the fp32 distance to the nearest valid face (+inf without a valid face);
+ *   m2p   area-weighted mean over 16 fixed quadrature points per valid face of the fp32 distance to the nearest cloud
+ *         point (+inf when the valid faces have zero total area);
+ *   nc_p, nc_m  the matching means of |normal . unit face normal| (0 where the distance is +inf).
+ * out_faces int32 [S][N]: valid faces per candidate.  Optional test outputs (NULL: not written; each pair both or
+ * neither): point_dist fp32 / point_face int32 [S][N][P] (nearest face, lowest index on ties; -1 without a valid face);
+ * quad_dist fp32 / quad_point int32 [S][N][F][16] (nearest cloud point, lowest index on ties; +inf / -1 on invalid
+ * faces).  ws: ma_mesh_score_workspace_bytes(S, N, F, P) bytes (no device needed; 0 for shapes out of range: S, N, F,
+ * P >= 1, S N <= 65535).  Fixed-order fp64 reductions without atomics: two calls give identical bits. */
+size_t ma_mesh_score_workspace_bytes(int S, int N, int F, int P);
+int ma_mesh_score(const float* meshes, const float* clouds, int S, int N, int F, int P, double* out,
+                  int32_t* out_faces, float* point_dist, int32_t* point_face, float* quad_dist, int32_t* quad_point,
+                  void* ws, void* stream);
+
 /* number of kernels launched by the library since load (bench.py's gpu_launches) */
 unsigned long long ma_launch_count(void);
 

@@ -77,7 +77,20 @@ def get_args():
     # not in the reference: run this rank's shapes through `batchsize_per_gpu` decoder cache slots, refilling a slot as
     # soon as its mesh is complete, instead of padded batches (SURVEY.md section 8(f)2; MeshAnything.forward_queue)
     parser.add_argument('--continuous_batching', default=False, action="store_true")
+    # not in the reference: sample N meshes of every shape in one batch and keep the one closest to the input cloud
+    # (Chamfer distance on the GPU; MeshAnything.forward_candidates) instead of re-rolling --seed by hand
+    parser.add_argument('--num_samples', default=1, type=int)
     return parser.parse_args()
+
+
+def check_args(args):
+    if args.num_samples < 1:
+        raise ValueError(f"--num_samples must be >= 1, got {args.num_samples}")
+    if args.num_samples > 1 and not args.sampling:
+        raise ValueError("--num_samples > 1 needs --sampling: greedy decoding gives the same mesh every time")
+    if args.num_samples > 1 and args.continuous_batching:
+        raise ValueError("--num_samples > 1 does not run with --continuous_batching: best-of-N scores the candidates "
+                         "of a padded batch together")
 
 
 def load_model(args, device=None):
@@ -176,6 +189,7 @@ def export_obj(path, faces_xyz):
 
 if __name__ == "__main__":
     args = get_args()
+    check_args(args)
     from meshanything_b200 import parallel
     rank, world, local = parallel.init_from_env()
     cur_time = datetime.datetime.now().strftime("%d_%H-%M-%S")
@@ -223,6 +237,16 @@ if __name__ == "__main__":
             continue
         items = [dataset[i] for i in idxs]
         pc = torch.from_numpy(np.stack([it['pc_normal'] for it in items]))
+        if args.num_samples > 1:
+            res = model.forward_candidates(pc, args.num_samples)
+            chamfer, nc, index = res.chamfer.cpu().tolist(), res.normal_consistency.cpu().tolist(), res.index.tolist()
+            for batch_id, it in enumerate(items):
+                for k in range(args.num_samples):
+                    kept = "  <- kept" if k == index[batch_id] else ""
+                    print(f"{it['uid']} sample {k}: chamfer {chamfer[batch_id][k]:.6f} "
+                          f"normal consistency {nc[batch_id][k]:.4f}{kept}")
+                save(it, res.best[batch_id])
+            continue
         outputs = model(pc, sampling=args.sampling)
         for batch_id, it in enumerate(items):
             save(it, outputs[batch_id])

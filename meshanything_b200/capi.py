@@ -46,6 +46,7 @@ EXPORTS = [
     "ma_mega_set_debug", "ma_linear_ws_set_mode", "ma_decode_slots_seek", "ma_decode_slot_stream", "ma_linear_ws_scratch_bytes", "ma_linear_ws_f16",
     "ma_sample_surface_workspace_bytes", "ma_sample_surface", "ma_tensor_core_linear_counts", "ma_decode_persistent_supported",
     "ma_udf_grid", "ma_marching_cubes_workspace_bytes", "ma_marching_cubes_count", "ma_marching_cubes_emit",
+    "ma_mesh_score_workspace_bytes", "ma_mesh_score",
 ]
 
 
@@ -119,6 +120,9 @@ def lib():
     L.ma_marching_cubes_workspace_bytes.restype = C.c_size_t
     L.ma_marching_cubes_count.argtypes = [_vp, C.c_int, C.c_float, _vp, C.POINTER(C.c_int64), _vp]
     L.ma_marching_cubes_emit.argtypes = [_vp, C.c_int, C.c_float, _vp, _vp, _vp, _vp]
+    L.ma_mesh_score_workspace_bytes.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
+    L.ma_mesh_score_workspace_bytes.restype = C.c_size_t
+    L.ma_mesh_score.argtypes = [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]
     L.ma_linear_tc_f16.argtypes = [_vp, _vp, _vp, C.c_int, _vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _vp]
     L.ma_set_tensor_cores.argtypes = [C.c_int]
     L.ma_tensor_core_linear_counts.argtypes = [C.POINTER(C.c_ulonglong), C.POINTER(C.c_ulonglong)]
@@ -217,6 +221,41 @@ def marching_cubes(field: torch.Tensor, level: float):
     check(lib().ma_marching_cubes_emit(ptr(fld), n, C.c_float(level), ptr(ws), ptr(verts), ptr(tris), stream_ptr()),
           "ma_marching_cubes_emit")
     return verts, tris
+
+
+def mesh_score(meshes: torch.Tensor, clouds: torch.Tensor, want_terms: bool = False):
+    """Chamfer terms of S x N candidate meshes against their clouds (ma_mesh_score; metrics.score adds the frame map).
+
+    meshes fp32 [S, N, F, 3, 3] (NaN rows = absent faces), clouds fp32 [S, P, 6] already in the output frame.
+    Returns (terms fp64 [S, N, 4] = p2m, m2p, nc_p, nc_m; valid faces int32 [S, N]); with want_terms also the
+    per-point (distance fp32 [S, N, P], face int32) and per-quadrature-point (distance fp32 [S, N, F, 16], cloud index
+    int32) results."""
+    _need_cuda(meshes, clouds)
+    m = meshes.to(torch.float32).contiguous()
+    c = clouds.to(torch.float32).contiguous()
+    if m.dim() != 5 or tuple(m.shape[3:]) != (3, 3) or c.dim() != 3 or c.shape[2] != 6 or c.shape[0] != m.shape[0]:
+        raise ValueError("mesh_score: meshes [S, N, F, 3, 3] and clouds [S, P, 6]")
+    S, N, F = m.shape[:3]
+    P = c.shape[1]
+    if min(S, N, F, P) < 1 or S * N > 65535:
+        raise ValueError("mesh_score: S, N, F, P >= 1 and S * N <= 65535")
+    if m.device != c.device:
+        raise ValueError("mesh_score: meshes and clouds on different devices")
+    if not bool(torch.isfinite(c).all()):
+        raise ValueError("mesh_score: non-finite cloud")
+    if not bool(torch.isfinite(m[~torch.isnan(m[..., 0, 0])]).all()):
+        raise ValueError("mesh_score: non-finite coordinates in a valid face (only a NaN first coordinate marks a face "
+                         "absent)")
+    dev = m.device
+    ws = torch.empty(lib().ma_mesh_score_workspace_bytes(S, N, F, P), dtype=torch.uint8, device=dev)
+    out = torch.empty((S, N, 4), dtype=torch.float64, device=dev)
+    faces = torch.empty((S, N), dtype=torch.int32, device=dev)
+    extra = (torch.empty((S, N, P), dtype=torch.float32, device=dev), torch.empty((S, N, P), dtype=torch.int32, device=dev),
+             torch.empty((S, N, F, 16), dtype=torch.float32, device=dev),
+             torch.empty((S, N, F, 16), dtype=torch.int32, device=dev)) if want_terms else (None,) * 4
+    check(lib().ma_mesh_score(ptr(m), ptr(c), S, N, F, P, ptr(out), ptr(faces), *[ptr(t) for t in extra], ptr(ws),
+                              stream_ptr()), "ma_mesh_score")
+    return (out, faces, *extra) if want_terms else (out, faces)
 
 
 def tensor_core_linear_counts():

@@ -19,47 +19,11 @@
 #include "canon.cuh"
 #include "internal.h"
 #include "mc_table.h"
+#include "tri_dist.cuh"
 
 namespace ma {
 
-// ---------------------------------------------------------------- (a) distance field
-
-struct wt_v3 { float x, y, z; };
-
-__device__ __forceinline__ wt_v3 wt_sub(wt_v3 a, wt_v3 b) {
-  return {__fsub_rn(a.x, b.x), __fsub_rn(a.y, b.y), __fsub_rn(a.z, b.z)};
-}
-__device__ __forceinline__ float wt_dot(wt_v3 a, wt_v3 b) {
-  return __fadd_rn(__fadd_rn(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)), __fmul_rn(a.z, b.z));
-}
-__device__ __forceinline__ wt_v3 wt_cross(wt_v3 a, wt_v3 b) {
-  return {__fsub_rn(__fmul_rn(a.y, b.z), __fmul_rn(a.z, b.y)), __fsub_rn(__fmul_rn(a.z, b.x), __fmul_rn(a.x, b.z)),
-          __fsub_rn(__fmul_rn(a.x, b.y), __fmul_rn(a.y, b.x))};
-}
-// squared distance from the point w (relative to the segment's start) to the segment [0, e]; a zero-length segment is
-// its point
-__device__ __forceinline__ float wt_seg2(wt_v3 w, wt_v3 e) {
-  const float l = wt_dot(e, e);
-  float t = l > 0.0f ? __fdiv_rn(wt_dot(w, e), l) : 0.0f;
-  t = fminf(fmaxf(t, 0.0f), 1.0f);
-  const wt_v3 q = {__fsub_rn(w.x, __fmul_rn(t, e.x)), __fsub_rn(w.y, __fmul_rn(t, e.y)), __fsub_rn(w.z, __fmul_rn(t, e.z))};
-  return wt_dot(q, q);
-}
-// Euclidean distance from p to the triangle (a, b, c): the plane distance when p projects inside the triangle (all
-// three edge tests >= 0), else the nearest of the three edges.  A degenerate face (zero normal) is its segments.
-__device__ __forceinline__ float wt_tri_dist(wt_v3 p, wt_v3 a, wt_v3 b, wt_v3 c) {
-  const wt_v3 ab = wt_sub(b, a), bc = wt_sub(c, b), ca = wt_sub(a, c);
-  const wt_v3 ap = wt_sub(p, a), bp = wt_sub(p, b), cp = wt_sub(p, c);
-  const wt_v3 nrm = wt_cross(ab, wt_sub(c, a));
-  const float nn = wt_dot(nrm, nrm);
-  if (nn > 0.0f && wt_dot(wt_cross(ab, ap), nrm) >= 0.0f && wt_dot(wt_cross(bc, bp), nrm) >= 0.0f &&
-      wt_dot(wt_cross(ca, cp), nrm) >= 0.0f) {
-    const float h = wt_dot(ap, nrm);
-    return __fsqrt_rn(__fdiv_rn(__fmul_rn(h, h), nn));
-  }
-  const float d2 = fminf(fminf(wt_seg2(ap, ab), wt_seg2(bp, bc)), wt_seg2(cp, ca));
-  return __fsqrt_rn(d2);
-}
+// ---------------------------------------------------------------- (a) distance field (wt_tri_dist: tri_dist.cuh)
 
 __global__ void udf_fill_kernel(float* __restrict__ field, size_t count, float band) {
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < count; i += (size_t)gridDim.x * blockDim.x)
