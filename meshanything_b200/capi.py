@@ -268,26 +268,40 @@ def tensor_core_linear_counts():
 _ws_scratch = {}
 
 
-def linear_ws_f16(w: torch.Tensor, bias: Optional[torch.Tensor], x: torch.Tensor, epilogue: int = EPI_NONE) -> torch.Tensor:
-    """fp16(x @ w.T + bias) for M <= 128 rows on the weight-streaming wgmma GEMM (hardware accumulation order)."""
+def _linear_out(out: Optional[torch.Tensor], M: int, N: int, device) -> torch.Tensor:
+    if out is None:
+        return torch.empty((M, N), dtype=torch.float16, device=device)
+    _need_cuda(out)
+    assert out.dtype == torch.float16 and out.shape == (M, N) and out.stride(1) == 1
+    return out
+
+
+def linear_ws_f16(w: torch.Tensor, bias: Optional[torch.Tensor], x: torch.Tensor, epilogue: int = EPI_NONE,
+                  out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """fp16(x @ w.T + bias) for M <= 128 rows on the weight-streaming wgmma GEMM (hardware accumulation order).
+    x and out may be row-strided views (a column slice of a wider buffer): their stride(0) is passed as ldx / ldy."""
     _need_cuda(w, bias, x)
+    assert x.dim() == 2 and x.stride(1) == 1
     M, K = x.shape
     N = w.shape[0]
     scr = _ws_scratch.get(x.device)
     if scr is None:
         scr = _ws_scratch[x.device] = torch.zeros(lib().ma_linear_ws_scratch_bytes(), dtype=torch.uint8, device=x.device)
-    out = torch.empty((M, N), dtype=torch.float16, device=x.device)
+    out = _linear_out(out, M, N, x.device)
     check(lib().ma_linear_ws_f16(ptr(w), ptr(bias), ptr(x), x.stride(0), ptr(out), out.stride(0), M, N, K, epilogue,
                                  ptr(scr), stream_ptr()), "ma_linear_ws_f16")
     return out
 
 
-def linear_tc_f16(w: torch.Tensor, bias: Optional[torch.Tensor], x: torch.Tensor, epilogue: int = EPI_NONE) -> torch.Tensor:
-    """fp16(x @ w.T + bias) on the wgmma tensor cores (hardware accumulation order)."""
+def linear_tc_f16(w: torch.Tensor, bias: Optional[torch.Tensor], x: torch.Tensor, epilogue: int = EPI_NONE,
+                  out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """fp16(x @ w.T + bias) on the wgmma tensor cores (hardware accumulation order).
+    x and out may be row-strided views (a column slice of a wider buffer): their stride(0) is passed as ldx / ldy."""
     _need_cuda(w, bias, x)
+    assert x.dim() == 2 and x.stride(1) == 1
     M, K = x.shape
     N = w.shape[0]
-    out = torch.empty((M, N), dtype=torch.float16, device=x.device)
+    out = _linear_out(out, M, N, x.device)
     check(lib().ma_linear_tc_f16(ptr(w), ptr(bias), ptr(x), x.stride(0), ptr(out), out.stride(0), M, N, K, epilogue,
                                  stream_ptr()), "ma_linear_tc_f16")
     return out

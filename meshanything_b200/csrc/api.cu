@@ -159,7 +159,8 @@ static int run_layers(const ma_decoder_weights* w, const DecWs& ws, void* kv, in
 struct GraphKey {
   const void *w, *kv, *ws, *out_ids, *forced, *logits_out;
   unsigned long long whash;
-  int B, tmax, max_new, bucket, flags, do_sample, top_k, eos, pad, mode;
+  // mode: generate (0) or slot (1) graphs; ws_mode: the gemm_ws reduction (linear_ws_mode()), which a graph bakes in
+  int B, tmax, max_new, bucket, flags, do_sample, top_k, eos, pad, mode, ws_mode;
   float top_p;
   unsigned long long seed;
   bool operator<(const GraphKey& o) const { return memcmp(this, &o, sizeof(GraphKey)) < 0; }
@@ -450,6 +451,7 @@ int ma_decode_generate(const ma_decoder_weights* w, const float* prefix, int B, 
       key.do_sample = sa.do_sample; key.top_k = sa.top_k; key.eos = eos_id; key.pad = pad_id; key.top_p = sa.top_p;
       key.seed = sa.do_sample ? sa.seed : 0;   // greedy graphs do not depend on the seed
       key.whash = whash;
+      key.ws_mode = linear_ws_mode();
       if (launch_cached_graph(key, st, enqueue)) return 1;
     }
     if (early && (i % CHECK_EVERY) == 0) {
@@ -599,7 +601,9 @@ int ma_decode_slots_step(const ma_decoder_weights* w, int B, int tmax, int max_n
       key.w = w; key.kv = kv; key.ws = ws_; key.out_ids = out_ids;
       key.B = B; key.tmax = tmax; key.max_new = max_new; key.bucket = bucket; key.flags = flags; key.mode = 1;
       key.do_sample = sa.do_sample; key.top_k = sa.top_k; key.eos = eos_id; key.pad = pad_id; key.top_p = sa.top_p;
-      key.seed = sa.do_sample ? sa.seed : 0;   // greedy graphs do not depend on the seed key.whash = whash;
+      key.seed = sa.do_sample ? sa.seed : 0;   // greedy graphs do not depend on the seed
+      key.whash = whash;
+      key.ws_mode = linear_ws_mode();
       if (launch_cached_graph(key, st, enqueue)) return 1;
     }
   }
