@@ -322,6 +322,25 @@ int ma_mesh_score(const float* meshes, const float* clouds, int S, int N, int F,
                   int32_t* out_faces, float* point_dist, int32_t* point_face, float* quad_dist, int32_t* quad_point,
                   void* ws, void* stream);
 
+/* ---- oriented normals of a bare point cloud (`--input_type pc`; csrc/normals.cu) -------------------------------
+ * xyz fp32 [n][3], finite, already in the output frame ((p - c) / L, metrics.to_output_frame) -> normals_out fp32
+ * [n][3] unit normals as DESIGN.md section 1.2 defines them: the k nearest other points under the key (fp32
+ * d^2 = (dx dx + dy dy) + dz dz, index), fp64 PCA of the point and its neighbours with 5 cyclic Jacobi sweeps, and
+ * orientation along the minimum spanning forest of the kNN graph under the edge order (max(0, 1 - |u_i . u_j|),
+ * min(i,j), max(i,j)) from the point of largest |p|^2 of each component, whose normal points away from the origin.
+ * Optional test outputs (NULL: not written): knn_out int32 [n][k] (rank order), unoriented_out fp32 [n][3].
+ * 1 <= k <= 64, k < n <= 2^24.  ws: ma_estimate_normals_workspace_bytes(n, k) bytes (needs the device: it sizes CUB's
+ * scan; 0 for shapes out of range).  Synchronises the stream once per Boruvka round (a 4-byte read-back).  Every
+ * choice is a minimum over unique keys: two calls give identical bits. */
+size_t ma_estimate_normals_workspace_bytes(int n, int k);
+int ma_estimate_normals(const float* xyz, int n, int k, float* normals_out, int32_t* knn_out, float* unoriented_out,
+                        void* ws, void* stream);
+/* Measurement hooks (tools/bench_normals.py): events = 5 cudaEvent_t recorded on the stream of every following call at
+ * its start and after the grid build, the kNN, the PCA and the orientation (NULL: off); the number of Boruvka rounds
+ * of the last call. */
+void ma_estimate_normals_set_events(void* const* events);
+int ma_estimate_normals_last_rounds(void);
+
 /* number of kernels launched by the library since load (bench.py's gpu_launches) */
 unsigned long long ma_launch_count(void);
 

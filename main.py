@@ -1,6 +1,7 @@
 """Drop-in for /root/reference/main.py (same flags, same outputs) on top of the H100-native MeshAnything.
 
     python main.py --input_type pc_normal --input_path pc_examples/mouse.npy --out_dir out [--sampling]
+    python main.py --input_type pc --input_path scan.npy       # bare (N, 3) cloud: normals estimated on the GPU
     torchrun --nproc-per-node 8 main.py --input_type pc_normal --input_dir pcs --batchsize_per_gpu 64
 
 Differences forced by the environment: no accelerate / hf_hub (there is no network) -- one process per
@@ -29,6 +30,21 @@ def _subsample_points(path, n_points=4096):
     return cloud[keep]
 
 
+def _points_with_normals(path, n_points=4096, k=16):
+    """`--input_type pc`: a bare cloud (.npy (N, 3) or vertex-only .ply) of >= 4096 points.  Normals are estimated on
+    the GPU from all N points (meshanything_b200.normals), then the same random 4096-subset as `pc_normal` is drawn: the
+    xyz-only copy of a file selects the points the file with normals selects under the same seed."""
+    from mesh_to_pc import load_points
+    from meshanything_b200.normals import estimate_normals
+    xyz = load_points(path)
+    if not np.issubdtype(xyz.dtype, np.floating):
+        xyz = xyz.astype(np.float64)
+    assert xyz.shape[0] >= n_points, "input pc_normal should have at least 4096 points"
+    normals = estimate_normals(xyz, k).cpu().numpy()
+    keep = np.random.choice(xyz.shape[0], n_points, replace=False)
+    return np.concatenate([xyz[keep], normals[keep].astype(xyz.dtype)], axis=1)
+
+
 def _uid_of(path):
     return path.split('/')[-1].split('.')[0]
 
@@ -40,6 +56,8 @@ class Dataset:
     def __init__(self, input_type, input_list, mc=False):
         if input_type == 'pc_normal':
             clouds = [_subsample_points(p) for p in input_list]
+        elif input_type == 'pc':
+            clouds = [_points_with_normals(p) for p in input_list]
         elif input_type == 'mesh':
             if mc:
                 print("First Marching Cubes and then sample point cloud, need several minutes...")
@@ -70,7 +88,8 @@ def get_args():
     parser = argparse.ArgumentParser("MeshAnything", add_help=False)
     for flag, default, typ in _FLAGS:
         parser.add_argument(flag, default=default, type=typ)
-    parser.add_argument('--input_type', choices=['mesh', 'pc_normal'], default='pc',
+    # 'pc' (the reference's default, which it does not implement): a bare (N, 3) cloud, normals estimated on the GPU
+    parser.add_argument('--input_type', choices=['mesh', 'pc_normal', 'pc'], default='pc',
                         help="Type of the asset to process (default: pc)")
     for switch in ('--mc', '--sampling'):
         parser.add_argument(switch, default=False, action="store_true")
@@ -203,6 +222,8 @@ if __name__ == "__main__":
         input_list = sorted(os.listdir(args.input_dir))
         if args.input_type == 'pc_normal':
             input_list = [os.path.join(args.input_dir, x) for x in input_list if x.endswith('.npy')]
+        elif args.input_type == 'pc':
+            input_list = [os.path.join(args.input_dir, x) for x in input_list if x.endswith('.npy') or x.endswith('.ply')]
         else:
             input_list = [os.path.join(args.input_dir, x) for x in input_list
                           if x.endswith('.ply') or x.endswith('.obj') or x.endswith('.npy')]

@@ -66,6 +66,14 @@ class SimpleMesh:
     def load_ply(path):
         """ASCII and binary (little/big endian) PLY: `vertex` (x, y, z among any other scalar properties) and `face`
         (one list property of vertex indices, polygons fan-triangulated).  Other elements are skipped."""
+        verts, faces = SimpleMesh._read_ply(path)
+        if verts is None or not faces:
+            raise ValueError(f"{path}: PLY without vertex/face elements (point clouds go through --input_type pc_normal)")
+        return SimpleMesh(verts, np.asarray(faces, dtype=np.int64))
+
+    @staticmethod
+    def _read_ply(path):
+        """(vertices float64 [V, 3] or None, list of triangles) of a PLY file."""
         T = SimpleMesh._PLY_TYPES
         with open(path, "rb") as f:
             if f.readline().strip() != b"ply":
@@ -123,9 +131,30 @@ class SimpleMesh:
                         ids = np.frombuffer(f.read(np.dtype(pr[3]).itemsize * k), dtype=end + pr[3]).astype(np.int64)
                         if el["name"] == "face":
                             faces.extend([ids[0], ids[j], ids[j + 1]] for j in range(1, k - 1))
-        if verts is None or not faces:
-            raise ValueError(f"{path}: PLY without vertex/face elements (point clouds go through --input_type pc_normal)")
-        return SimpleMesh(verts, np.asarray(faces, dtype=np.int64))
+        return verts, faces
+
+
+def load_points(path):
+    """A bare point cloud for `--input_type pc`: an .npy of shape (N, 3), or a .ply with a `vertex` element (x, y, z
+    among any other properties; ASCII or binary) and no faces.  Returns the xyz array ([N, 3]; the .npy's own dtype,
+    float64 from a PLY).  An (N, 6) .npy is refused rather than having its normals dropped."""
+    low = path.lower()
+    if low.endswith(".npy"):
+        xyz = np.load(path)
+        if xyz.ndim == 2 and xyz.shape[1] == 6:
+            raise ValueError(f"{path}: shape {xyz.shape} looks like points with normals; use --input_type pc_normal, "
+                             "which keeps them (--input_type pc estimates normals for bare (N, 3) clouds)")
+        if xyz.ndim != 2 or xyz.shape[1] != 3:
+            raise ValueError(f"{path}: a bare point cloud is an array of shape (N, 3), got {xyz.shape}")
+        return xyz
+    if low.endswith(".ply"):
+        verts, faces = SimpleMesh._read_ply(path)
+        if verts is None:
+            raise ValueError(f"{path}: PLY without a vertex element")
+        if faces:
+            raise ValueError(f"{path}: PLY with faces is a mesh; use --input_type mesh")
+        return verts
+    raise ValueError(f"{path}: --input_type pc reads .npy (N, 3) and vertex-only .ply files")
 
 
 def load_mesh(path):

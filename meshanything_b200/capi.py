@@ -47,6 +47,8 @@ EXPORTS = [
     "ma_sample_surface_workspace_bytes", "ma_sample_surface", "ma_tensor_core_linear_counts", "ma_decode_persistent_supported",
     "ma_udf_grid", "ma_marching_cubes_workspace_bytes", "ma_marching_cubes_count", "ma_marching_cubes_emit",
     "ma_mesh_score_workspace_bytes", "ma_mesh_score",
+    "ma_estimate_normals_workspace_bytes", "ma_estimate_normals", "ma_estimate_normals_set_events",
+    "ma_estimate_normals_last_rounds",
 ]
 
 
@@ -123,6 +125,13 @@ def lib():
     L.ma_mesh_score_workspace_bytes.argtypes = [C.c_int, C.c_int, C.c_int, C.c_int]
     L.ma_mesh_score_workspace_bytes.restype = C.c_size_t
     L.ma_mesh_score.argtypes = [_vp, _vp, C.c_int, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]
+    L.ma_estimate_normals_workspace_bytes.argtypes = [C.c_int, C.c_int]
+    L.ma_estimate_normals_workspace_bytes.restype = C.c_size_t
+    L.ma_estimate_normals.argtypes = [_vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp]
+    L.ma_estimate_normals_set_events.argtypes = [_vp]
+    L.ma_estimate_normals_set_events.restype = None
+    L.ma_estimate_normals_last_rounds.argtypes = []
+    L.ma_estimate_normals_last_rounds.restype = C.c_int
     L.ma_linear_tc_f16.argtypes = [_vp, _vp, _vp, C.c_int, _vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _vp]
     L.ma_set_tensor_cores.argtypes = [C.c_int]
     L.ma_tensor_core_linear_counts.argtypes = [C.POINTER(C.c_ulonglong), C.POINTER(C.c_ulonglong)]
@@ -256,6 +265,31 @@ def mesh_score(meshes: torch.Tensor, clouds: torch.Tensor, want_terms: bool = Fa
     check(lib().ma_mesh_score(ptr(m), ptr(c), S, N, F, P, ptr(out), ptr(faces), *[ptr(t) for t in extra], ptr(ws),
                               stream_ptr()), "ma_mesh_score")
     return (out, faces, *extra) if want_terms else (out, faces)
+
+
+def estimate_normals(points: torch.Tensor, k: int = 16, want_terms: bool = False):
+    """Oriented unit normals of a bare cloud (ma_estimate_normals; normals.estimate_normals adds the frame map).
+
+    points fp32 [N, 3], finite, already in the output frame; 1 <= k <= 64, k < N <= 2^24.  Returns normals fp32 [N, 3];
+    with want_terms (normals, kNN int32 [N, k] in rank order, unoriented normals fp32 [N, 3])."""
+    _need_cuda(points)
+    p = points.to(torch.float32).contiguous()
+    if p.dim() != 2 or p.shape[1] != 3:
+        raise ValueError("estimate_normals: points [N, 3]")
+    n = p.shape[0]
+    if not 1 <= k <= 64:
+        raise ValueError(f"estimate_normals: 1 <= k <= 64, got k = {k}")
+    if not k < n <= 1 << 24:
+        raise ValueError(f"estimate_normals: k < N <= 2^24, got N = {n}, k = {k}")
+    if not bool(torch.isfinite(p).all()):
+        raise ValueError("estimate_normals: non-finite coordinates")
+    ws = torch.empty(lib().ma_estimate_normals_workspace_bytes(n, k), dtype=torch.uint8, device=p.device)
+    out = torch.empty((n, 3), dtype=torch.float32, device=p.device)
+    knn = torch.empty((n, k), dtype=torch.int32, device=p.device) if want_terms else None
+    uno = torch.empty((n, 3), dtype=torch.float32, device=p.device) if want_terms else None
+    check(lib().ma_estimate_normals(ptr(p), n, k, ptr(out), ptr(knn), ptr(uno), ptr(ws), stream_ptr()),
+          "ma_estimate_normals")
+    return (out, knn, uno) if want_terms else out
 
 
 def tensor_core_linear_counts():

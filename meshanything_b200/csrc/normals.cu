@@ -1,0 +1,501 @@
+// normals.cu -- oriented normals of a bare point cloud for `--input_type pc` (DESIGN.md section 1.2 defines them).
+//
+// The points arrive already in the output frame (p' = (p - c) / L, metrics.to_output_frame), fp32 [N][3].
+//   (a) grid      normals_cell_kernel counts the points per cell of a G^3 grid over [-0.5, 0.5]^3, a CUB exclusive
+//                 scan gives the cell starts, normals_scatter_kernel writes the points in cell order (float4: xyz and
+//                 the original index).  The order inside a cell is whatever the atomics give: nothing depends on it.
+//   (b) kNN       normals_knn_kernel, one thread per point: shells of cells by Chebyshev radius r = 0, 1, ... around
+//                 the query's cell, every candidate keyed by (fp32 d^2 bits << 32 | index), the k smallest keys kept
+//                 sorted in shared memory.  After shell r it stops when the k-th key's d^2 is below a lower bound of
+//                 the distance to every cell outside the shells (shrunk by a margin far above fp32 rounding), or when
+//                 no cell is left.  The grid size therefore only changes the speed: the result is the exact kNN.
+//   (c) PCA       normals_pca_kernel, one thread per point: fp64 centroid and covariance of the point and its
+//                 neighbours in rank order, sequential sums of explicit __d*_rn operations, then kNmSweeps cyclic
+//                 Jacobi sweeps; the eigenvector of the smallest diagonal entry, normalised in fp64, rounded to fp32.
+//   (d) orient    Boruvka over the kNN graph.  Each vertex carries a word (component root << 1 | parity), the parity
+//                 being its sign relative to that root.  A round: every component's minimum outgoing edge under the
+//                 strict order (w, min(i,j), max(i,j)) by two 64/32-bit atomicMin passes over unique keys; each
+//                 component hooks onto the component across that edge (of a mutual pair the larger root hooks) with
+//                 parity = parity(x) ^ parity(y) ^ (u_x . u_y < 0); pointer jumping on single 32-bit words composes
+//                 parities by XOR; every vertex is relabelled.  One 4-byte read-back per round (the number of hooks)
+//                 decides whether another round runs.  Finally the point of largest |p'|^2 (lowest index on ties) of
+//                 each component fixes the component's sign.
+// Every fp32 step is an explicit round-to-nearest intrinsic, every fp64 step too (nvcc contracts fp64 as well), and
+// every choice is a minimum over unique keys, so a call is bit-deterministic and tests/normals_oracle.py restates the
+// neighbours, the unoriented and the oriented normals bit for bit.
+#include <cub/device/device_scan.cuh>
+
+#include "canon.cuh"
+#include "internal.h"
+
+namespace ma {
+
+constexpr int kNmThreads = 256;
+constexpr int kNmKnnThreads = 64;   // kNN threads per CTA: k x 64 x 8 B of shared memory for the top-k lists
+constexpr int kNmSweeps = 5;        // Jacobi sweeps: 4 reach 4e-15 rad against LAPACK on separated spectra, 1 spare
+constexpr int kNmMaxK = 64;
+constexpr int kNmMaxN = 1 << 24;    // vertex words hold the root in 31 bits; the index part of a kNN key in 32
+constexpr int kNmMaxG = 256;
+constexpr int kNmMaxRounds = 64;    // Boruvka at least halves the components with an outgoing edge per round
+
+// grid cells per axis: about 4 k points per occupied cell of a surface, so that radius 1 mostly suffices
+static int nm_grid(int n, int k) {
+  const int g = (int)ceil(0.5 * sqrt((double)n / (double)k));
+  return std::max(1, std::min(kNmMaxG, g));
+}
+
+__device__ __forceinline__ int nm_cell1(float x, int G) {
+  const int c = (int)floorf(__fmul_rn(__fadd_rn(x, 0.5f), (float)G));
+  return min(max(c, 0), G - 1);
+}
+
+__device__ __forceinline__ float nm_dot(float ax, float ay, float az, float bx, float by, float bz) {
+  return __fadd_rn(__fadd_rn(__fmul_rn(ax, bx), __fmul_rn(ay, by)), __fmul_rn(az, bz));
+}
+
+// ---------------------------------------------------------------- (a) grid
+
+__global__ void normals_cell_kernel(const float* __restrict__ xyz, int n, int G, uint32_t* __restrict__ cell,
+                                    uint32_t* __restrict__ count) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float* p = xyz + 3 * (size_t)i;
+  const uint32_t c = ((uint32_t)nm_cell1(p[0], G) * G + nm_cell1(p[1], G)) * G + nm_cell1(p[2], G);
+  cell[i] = c;
+  atomicAdd(count + c, 1u);
+}
+
+// count[c] is used up as a cursor: the point takes slot start[c] + (atomicSub's old value - 1)
+__global__ void normals_scatter_kernel(const float* __restrict__ xyz, int n, const uint32_t* __restrict__ cell,
+                                       const uint32_t* __restrict__ start, uint32_t* __restrict__ count,
+                                       float4* __restrict__ sorted) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint32_t c = cell[i];
+  const uint32_t slot = start[c] + atomicSub(count + c, 1u) - 1u;
+  const float* p = xyz + 3 * (size_t)i;
+  sorted[slot] = make_float4(p[0], p[1], p[2], __int_as_float(i));
+}
+
+// ---------------------------------------------------------------- (b) exact kNN
+
+__global__ void __launch_bounds__(kNmKnnThreads) normals_knn_kernel(const float4* __restrict__ sorted,
+                                                                    const uint32_t* __restrict__ start, int n, int k,
+                                                                    int G, int32_t* __restrict__ knn) {
+  extern __shared__ unsigned long long nm_top[];  // [k][kNmKnnThreads]: entry e of thread t at e * 64 + t
+  const int s = blockIdx.x * kNmKnnThreads + threadIdx.x;
+  if (s >= n) return;
+  unsigned long long* top = nm_top + threadIdx.x;
+  const float4 q = sorted[s];
+  const int self = __float_as_int(q.w);
+  const int cx = nm_cell1(q.x, G), cy = nm_cell1(q.y, G), cz = nm_cell1(q.z, G);
+  const float inv = 1.0f / (float)G;
+  int m = 0;
+  for (int r = 0;; r++) {
+    for (int dx = -r; dx <= r; dx++) {
+      const int x = cx + dx;
+      if (x < 0 || x >= G) continue;
+      for (int dy = -r; dy <= r; dy++) {
+        const int y = cy + dy;
+        if (y < 0 || y >= G) continue;
+        // the shell of radius r: whole z columns on its x / y faces, only dz = -r and +r inside them
+        const int step = (r == 0 || dx == -r || dx == r || dy == -r || dy == r) ? 1 : 2 * r;
+        for (int dz = -r; dz <= r; dz += step) {
+          const int z = cz + dz;
+          if (z < 0 || z >= G) continue;
+          const uint32_t c = ((uint32_t)x * G + y) * G + z;
+          const uint32_t e1 = start[c + 1];
+          for (uint32_t t = start[c]; t < e1; t++) {
+            const float4 p = sorted[t];
+            const int j = __float_as_int(p.w);
+            if (j == self) continue;
+            const float ex = __fsub_rn(q.x, p.x), ey = __fsub_rn(q.y, p.y), ez = __fsub_rn(q.z, p.z);
+            const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)), __fmul_rn(ez, ez));
+            const unsigned long long key = ((unsigned long long)__float_as_uint(d2) << 32) | (uint32_t)j;
+            if (m == k && key >= top[(size_t)(k - 1) * kNmKnnThreads]) continue;
+            int e = m < k ? m++ : k - 1;
+            while (e > 0 && top[(size_t)(e - 1) * kNmKnnThreads] > key) {
+              top[(size_t)e * kNmKnnThreads] = top[(size_t)(e - 1) * kNmKnnThreads];
+              e--;
+            }
+            top[(size_t)e * kNmKnnThreads] = key;
+          }
+        }
+      }
+    }
+    // lower bound of the distance from q to any cell outside the cube [c - r, c + r]^3 (only the sides that have cells)
+    float b = INFINITY;
+    if (cx - r > 0) b = fminf(b, q.x - ((float)(cx - r) * inv - 0.5f));
+    if (cx + r < G - 1) b = fminf(b, ((float)(cx + r + 1) * inv - 0.5f) - q.x);
+    if (cy - r > 0) b = fminf(b, q.y - ((float)(cy - r) * inv - 0.5f));
+    if (cy + r < G - 1) b = fminf(b, ((float)(cy + r + 1) * inv - 0.5f) - q.y);
+    if (cz - r > 0) b = fminf(b, q.z - ((float)(cz - r) * inv - 0.5f));
+    if (cz + r < G - 1) b = fminf(b, ((float)(cz + r + 1) * inv - 0.5f) - q.z);
+    if (b == INFINITY) break;  // every cell has been searched
+    if (m == k) {
+      // margin: a point can sit ~1e-7 outside its cell after fp32 rounding, and d^2 carries a few ulps of error; a
+      // strict < because an unseen point at the same d^2 with a lower index would still rank first
+      const float bs = fmaxf(b - 1e-6f, 0.0f);
+      if (__uint_as_float((uint32_t)(top[(size_t)(k - 1) * kNmKnnThreads] >> 32)) < bs * bs * (1.0f - 1e-5f)) break;
+    }
+  }
+  int32_t* out = knn + (size_t)self * k;
+  for (int e = 0; e < k; e++) out[e] = (int32_t)(uint32_t)top[(size_t)e * kNmKnnThreads];
+}
+
+// ---------------------------------------------------------------- (c) PCA + Jacobi
+
+__global__ void normals_pca_kernel(const float* __restrict__ xyz, const int32_t* __restrict__ knn, int n, int k,
+                                   float* __restrict__ uno) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int32_t* nb = knn + (size_t)i * k;
+  const float* pi = xyz + 3 * (size_t)i;
+  double sx = pi[0], sy = pi[1], sz = pi[2];
+  for (int e = 0; e < k; e++) {
+    const float* pj = xyz + 3 * (size_t)nb[e];
+    sx = __dadd_rn(sx, (double)pj[0]);
+    sy = __dadd_rn(sy, (double)pj[1]);
+    sz = __dadd_rn(sz, (double)pj[2]);
+  }
+  const double cnt = (double)(k + 1);
+  const double mx = __ddiv_rn(sx, cnt), my = __ddiv_rn(sy, cnt), mz = __ddiv_rn(sz, cnt);
+  double c[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+  for (int e = -1; e < k; e++) {
+    const float* pj = e < 0 ? pi : xyz + 3 * (size_t)nb[e];
+    const double dx = __dsub_rn((double)pj[0], mx), dy = __dsub_rn((double)pj[1], my), dz = __dsub_rn((double)pj[2], mz);
+    const double t[6] = {__dmul_rn(dx, dx), __dmul_rn(dx, dy), __dmul_rn(dx, dz),
+                         __dmul_rn(dy, dy), __dmul_rn(dy, dz), __dmul_rn(dz, dz)};
+    if (e < 0) {
+#pragma unroll
+      for (int a = 0; a < 6; a++) c[a] = t[a];
+    } else {
+#pragma unroll
+      for (int a = 0; a < 6; a++) c[a] = __dadd_rn(c[a], t[a]);
+    }
+  }
+  double A[3][3] = {{c[0], c[1], c[2]}, {c[1], c[3], c[4]}, {c[2], c[4], c[5]}};
+  double V[3][3] = {{1.0, 0.0, 0.0}, {0.0, 1.0, 0.0}, {0.0, 0.0, 1.0}};
+  for (int sweep = 0; sweep < kNmSweeps; sweep++) {
+#pragma unroll
+    for (int pr = 0; pr < 3; pr++) {
+      const int p = pr == 2 ? 1 : 0, q = pr == 0 ? 1 : 2, r = 2 - pr;
+      const double apq = A[p][q];
+      if (apq == 0.0) continue;
+      const double app = A[p][p], aqq = A[q][q];
+      const double theta = __ddiv_rn(__dsub_rn(aqq, app), __dmul_rn(2.0, apq));
+      double t = __ddiv_rn(1.0, __dadd_rn(fabs(theta), __dsqrt_rn(__dadd_rn(__dmul_rn(theta, theta), 1.0))));
+      if (theta < 0.0) t = -t;
+      const double cs = __ddiv_rn(1.0, __dsqrt_rn(__dadd_rn(__dmul_rn(t, t), 1.0)));
+      const double sn = __dmul_rn(t, cs);
+      const double tapq = __dmul_rn(t, apq);
+      const double arp = A[r][p], arq = A[r][q];
+      A[p][p] = __dsub_rn(app, tapq);
+      A[q][q] = __dadd_rn(aqq, tapq);
+      A[p][q] = A[q][p] = 0.0;
+      A[r][p] = A[p][r] = __dsub_rn(__dmul_rn(cs, arp), __dmul_rn(sn, arq));
+      A[r][q] = A[q][r] = __dadd_rn(__dmul_rn(sn, arp), __dmul_rn(cs, arq));
+#pragma unroll
+      for (int row = 0; row < 3; row++) {
+        const double vp = V[row][p], vq = V[row][q];
+        V[row][p] = __dsub_rn(__dmul_rn(cs, vp), __dmul_rn(sn, vq));
+        V[row][q] = __dadd_rn(__dmul_rn(sn, vp), __dmul_rn(cs, vq));
+      }
+    }
+  }
+  // the column of the smallest diagonal entry, the lowest column on ties
+  double v0 = V[0][0], v1 = V[1][0], v2 = V[2][0], dmin = A[0][0];
+  if (A[1][1] < dmin) { v0 = V[0][1]; v1 = V[1][1]; v2 = V[2][1]; dmin = A[1][1]; }
+  if (A[2][2] < dmin) { v0 = V[0][2]; v1 = V[1][2]; v2 = V[2][2]; }
+  const double ln = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(v0, v0), __dmul_rn(v1, v1)), __dmul_rn(v2, v2)));
+  float* o = uno + 3 * (size_t)i;
+  o[0] = (float)__ddiv_rn(v0, ln);
+  o[1] = (float)__ddiv_rn(v1, ln);
+  o[2] = (float)__ddiv_rn(v2, ln);
+}
+
+// ---------------------------------------------------------------- (d) orientation
+
+constexpr uint32_t kNmDead = 0xffffffffu;  // weight bits of a kNN slot whose endpoints share a component for good
+
+// w[slot] = bits of max(0, 1 - |u_i . u_j|); word[i] = i << 1 (own root, parity 0)
+__global__ void normals_weight_kernel(const float* __restrict__ uno, const int32_t* __restrict__ knn, int n, int k,
+                                      uint32_t* __restrict__ w, uint32_t* __restrict__ word) {
+  const size_t e = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (e >= (size_t)n * k) return;
+  const int i = (int)(e / k), j = knn[e];
+  const float* a = uno + 3 * (size_t)i;
+  const float* b = uno + 3 * (size_t)j;
+  const float d = nm_dot(a[0], a[1], a[2], b[0], b[1], b[2]);
+  w[e] = __float_as_uint(fmaxf(0.0f, __fsub_rn(1.0f, fabsf(d))));
+  if (e % k == 0) word[i] = (uint32_t)i << 1;
+}
+
+__global__ void normals_clear_kernel(int n, unsigned long long* __restrict__ best1, uint32_t* __restrict__ best2) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  best1[i] = ~0ull;
+  best2[i] = ~0u;
+}
+
+// pass 1: per component the least (w, min(i,j)) over its outgoing slots; slots found internal are marked dead
+__global__ void normals_min1_kernel(const int32_t* __restrict__ knn, int n, int k, uint32_t* __restrict__ w,
+                                    const uint32_t* __restrict__ word, unsigned long long* __restrict__ best1) {
+  const size_t e = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (e >= (size_t)n * k) return;
+  const uint32_t wb = w[e];
+  if (wb == kNmDead) return;
+  const uint32_t i = (uint32_t)(e / k), j = (uint32_t)knn[e];
+  const uint32_t ci = word[i] >> 1, cj = word[j] >> 1;
+  if (ci == cj) {
+    w[e] = kNmDead;
+    return;
+  }
+  const unsigned long long key = ((unsigned long long)wb << 32) | min(i, j);
+  atomicMin(best1 + ci, key);
+  atomicMin(best1 + cj, key);
+}
+
+// pass 2: among the slots that carry the winning (w, min) key, the least max(i,j)
+__global__ void normals_min2_kernel(const int32_t* __restrict__ knn, int n, int k, const uint32_t* __restrict__ w,
+                                    const uint32_t* __restrict__ word, const unsigned long long* __restrict__ best1,
+                                    uint32_t* __restrict__ best2) {
+  const size_t e = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  if (e >= (size_t)n * k) return;
+  const uint32_t wb = w[e];
+  if (wb == kNmDead) return;
+  const uint32_t i = (uint32_t)(e / k), j = (uint32_t)knn[e];
+  const uint32_t ci = word[i] >> 1, cj = word[j] >> 1;
+  const unsigned long long key = ((unsigned long long)wb << 32) | min(i, j);
+  if (key == best1[ci]) atomicMin(best2 + ci, max(i, j));
+  if (key == best1[cj]) atomicMin(best2 + cj, max(i, j));
+}
+
+// per root c: hook[c] = (new parent << 1) | parity of c relative to it; hook[c] = c << 1 when c stays a root
+__global__ void normals_hook_kernel(const float* __restrict__ uno, int n, const uint32_t* __restrict__ word,
+                                    const unsigned long long* __restrict__ best1, const uint32_t* __restrict__ best2,
+                                    uint32_t* __restrict__ hook, int* __restrict__ hooks) {
+  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= (uint32_t)n || (word[c] >> 1) != c) return;
+  const unsigned long long b1 = best1[c];
+  if (b1 == ~0ull) {
+    hook[c] = c << 1;
+    return;
+  }
+  const uint32_t a = (uint32_t)b1, b = best2[c];
+  const uint32_t x = (word[a] >> 1) == c ? a : b, y = x == a ? b : a;
+  const uint32_t d = word[y] >> 1;
+  if (best1[d] == b1 && best2[d] == b && c < d) {  // both chose this edge: the smaller root stays
+    hook[c] = c << 1;
+    return;
+  }
+  const float* ux = uno + 3 * (size_t)x;
+  const float* uy = uno + 3 * (size_t)y;
+  const uint32_t flip = nm_dot(ux[0], ux[1], ux[2], uy[0], uy[1], uy[2]) < 0.0f ? 1u : 0u;
+  hook[c] = (d << 1) | ((word[x] ^ word[y] ^ flip) & 1u);
+  atomicAdd(hooks, 1);
+}
+
+// pointer jumping over the hook forest.  Each root only writes its own word, and any word it reads is a valid
+// (ancestor, parity relative to it) pair, old or new: the result does not depend on the schedule.
+__global__ void normals_jump_kernel(int n, const uint32_t* __restrict__ word, uint32_t* hook) {
+  const uint32_t c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= (uint32_t)n || (word[c] >> 1) != c) return;
+  volatile uint32_t* h = hook;
+  uint32_t w = h[c];
+  for (;;) {
+    const uint32_t p = w >> 1, wp = h[p];
+    if ((wp >> 1) == p) break;
+    w = (wp & ~1u) | ((w ^ wp) & 1u);
+    h[c] = w;
+  }
+}
+
+__global__ void normals_relabel_kernel(int n, const uint32_t* __restrict__ hook, uint32_t* __restrict__ word) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= n) return;
+  const uint32_t w = word[v], r = hook[w >> 1];
+  word[v] = (r & ~1u) | ((w ^ r) & 1u);
+}
+
+// per component the point of largest fp32 |p|^2, lowest index on ties: max of (bits << 32 | ~index)
+__global__ void normals_far_kernel(const float* __restrict__ xyz, int n, const uint32_t* __restrict__ word,
+                                   unsigned long long* __restrict__ far) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= n) return;
+  const float* p = xyz + 3 * (size_t)v;
+  const float r2 = nm_dot(p[0], p[1], p[2], p[0], p[1], p[2]);
+  atomicMax(far + (word[v] >> 1), ((unsigned long long)__float_as_uint(r2) << 32) | (uint32_t)~(uint32_t)v);
+}
+
+__global__ void normals_apply_kernel(const float* __restrict__ xyz, const float* __restrict__ uno, int n,
+                                     const uint32_t* __restrict__ word, const unsigned long long* __restrict__ far,
+                                     float* __restrict__ out) {
+  const int v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= n) return;
+  const uint32_t wv = word[v];
+  const uint32_t f = ~(uint32_t)far[wv >> 1];
+  const float* uf = uno + 3 * (size_t)f;
+  const float* pf = xyz + 3 * (size_t)f;
+  const uint32_t neg = nm_dot(uf[0], uf[1], uf[2], pf[0], pf[1], pf[2]) < 0.0f ? 1u : 0u;
+  const bool flip = ((neg ^ word[f] ^ wv) & 1u) != 0;
+  const float* u = uno + 3 * (size_t)v;
+  out[3 * (size_t)v] = flip ? -u[0] : u[0];
+  out[3 * (size_t)v + 1] = flip ? -u[1] : u[1];
+  out[3 * (size_t)v + 2] = flip ? -u[2] : u[2];
+}
+
+// ---------------------------------------------------------------- workspace
+
+static size_t nm_align(size_t b) { return (b + 255) & ~(size_t)255; }
+static bool nm_shape_ok(int n, int k) { return k >= 1 && k <= kNmMaxK && n > k && n <= kNmMaxN; }
+
+static size_t nm_scan_bytes(size_t cells) {
+  size_t bytes = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, bytes, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)(cells + 1));
+  return bytes;
+}
+
+struct NmLayout {
+  size_t sorted, cell, count, start, scan, knn, uno, w, word, hook, best1, best2, hooks, total;
+};
+
+static NmLayout nm_layout(int n, int k) {
+  const int G = nm_grid(n, k);
+  const size_t cells = (size_t)G * G * G, nk = (size_t)n * k;
+  NmLayout L;
+  size_t o = 0;
+  auto take = [&](size_t bytes) { const size_t at = o; o += nm_align(bytes); return at; };
+  L.sorted = take((size_t)n * sizeof(float4));
+  L.cell = take((size_t)n * 4);
+  L.count = take((cells + 1) * 4);
+  L.start = take((cells + 1) * 4);
+  L.scan = take(nm_scan_bytes(cells));
+  L.knn = take(nk * 4);
+  L.uno = take((size_t)n * 12);
+  L.w = take(nk * 4);
+  L.word = take((size_t)n * 4);
+  L.hook = take((size_t)n * 4);
+  L.best1 = take((size_t)n * 8);
+  L.best2 = take((size_t)n * 4);
+  L.hooks = take(4);
+  L.total = o;
+  return L;
+}
+
+static cudaEvent_t g_nm_events[5];
+static bool g_nm_timed = false;
+static int g_nm_rounds = 0;
+
+static void nm_mark(int at, cudaStream_t st) {
+  if (g_nm_timed) cudaEventRecord(g_nm_events[at], st);
+}
+
+static int nm_blocks(size_t count) { return (int)((count + kNmThreads - 1) / kNmThreads); }
+
+}  // namespace ma
+
+using namespace ma;
+
+extern "C" {
+
+size_t ma_estimate_normals_workspace_bytes(int n, int k) {
+  if (!nm_shape_ok(n, k)) return 0;
+  return nm_layout(n, k).total;
+}
+
+void ma_estimate_normals_set_events(void* const* events) {
+  g_nm_timed = events != nullptr;
+  if (events)
+    for (int i = 0; i < 5; i++) g_nm_events[i] = (cudaEvent_t)events[i];
+}
+
+int ma_estimate_normals_last_rounds(void) { return g_nm_rounds; }
+
+int ma_estimate_normals(const float* xyz, int n, int k, float* normals_out, int32_t* knn_out, float* unoriented_out,
+                        void* ws, void* stream) {
+  if (!xyz || !normals_out || !ws || !nm_shape_ok(n, k)) {
+    set_error("ma_estimate_normals: bad arguments (1 <= k <= %d, k < n <= 2^24)", kNmMaxK);
+    return 1;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  const NmLayout L = nm_layout(n, k);
+  char* base = reinterpret_cast<char*>(ws);
+  auto* sorted = reinterpret_cast<float4*>(base + L.sorted);
+  auto* cell = reinterpret_cast<uint32_t*>(base + L.cell);
+  auto* count = reinterpret_cast<uint32_t*>(base + L.count);
+  auto* start = reinterpret_cast<uint32_t*>(base + L.start);
+  int32_t* knn = knn_out ? knn_out : reinterpret_cast<int32_t*>(base + L.knn);
+  float* uno = unoriented_out ? unoriented_out : reinterpret_cast<float*>(base + L.uno);
+  auto* w = reinterpret_cast<uint32_t*>(base + L.w);
+  auto* word = reinterpret_cast<uint32_t*>(base + L.word);
+  auto* hook = reinterpret_cast<uint32_t*>(base + L.hook);
+  auto* best1 = reinterpret_cast<unsigned long long*>(base + L.best1);
+  auto* best2 = reinterpret_cast<uint32_t*>(base + L.best2);
+  auto* hooks = reinterpret_cast<int*>(base + L.hooks);
+  const int G = nm_grid(n, k);
+  const size_t cells = (size_t)G * G * G, nk = (size_t)n * k;
+
+  nm_mark(0, st);
+  cudaError_t e = cudaMemsetAsync(count, 0, (cells + 1) * 4, st);
+  if (e != cudaSuccess) {
+    set_error("ma_estimate_normals: %s", cudaGetErrorString(e));
+    return 1;
+  }
+  normals_cell_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(xyz, n, G, cell, count);
+  size_t scan_bytes = nm_scan_bytes(cells);
+  e = cub::DeviceScan::ExclusiveSum(base + L.scan, scan_bytes, count, start, (int)(cells + 1), st);
+  normals_scatter_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(xyz, n, cell, start, count, sorted);
+  count_launch(3);
+  nm_mark(1, st);
+  normals_knn_kernel<<<(n + kNmKnnThreads - 1) / kNmKnnThreads, kNmKnnThreads,
+                       (size_t)k * kNmKnnThreads * sizeof(unsigned long long), st>>>(sorted, start, n, k, G, knn);
+  nm_mark(2, st);
+  normals_pca_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(xyz, knn, n, k, uno);
+  nm_mark(3, st);
+  normals_weight_kernel<<<nm_blocks(nk), kNmThreads, 0, st>>>(uno, knn, n, k, w, word);
+  count_launch(3);
+  if (e != cudaSuccess || !check_launch("ma_estimate_normals")) {
+    if (e != cudaSuccess) set_error("ma_estimate_normals: %s", cudaGetErrorString(e));
+    return 1;
+  }
+  int rounds = 0;
+  for (;;) {
+    if (rounds == kNmMaxRounds) {
+      set_error("ma_estimate_normals: Boruvka did not finish in %d rounds", kNmMaxRounds);
+      return 1;
+    }
+    rounds++;
+    int merged = 0;
+    e = cudaMemsetAsync(hooks, 0, sizeof(int), st);
+    normals_clear_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(n, best1, best2);
+    normals_min1_kernel<<<nm_blocks(nk), kNmThreads, 0, st>>>(knn, n, k, w, word, best1);
+    normals_min2_kernel<<<nm_blocks(nk), kNmThreads, 0, st>>>(knn, n, k, w, word, best1, best2);
+    normals_hook_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(uno, n, word, best1, best2, hook, hooks);
+    normals_jump_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(n, word, hook);
+    normals_relabel_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(n, hook, word);
+    count_launch(6);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&merged, hooks, sizeof(int), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess || !check_launch("ma_estimate_normals")) {
+      if (e != cudaSuccess) set_error("ma_estimate_normals: %s", cudaGetErrorString(e));
+      cudaGetLastError();
+      return 1;
+    }
+    if (merged == 0) break;
+  }
+  g_nm_rounds = rounds;
+  // the last round hooked nothing, so best1 is free again: it collects each component's farthest point
+  e = cudaMemsetAsync(best1, 0, (size_t)n * 8, st);
+  normals_far_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(xyz, n, word, best1);
+  normals_apply_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(xyz, uno, n, word, best1, normals_out);
+  count_launch(2);
+  nm_mark(4, st);
+  if (e != cudaSuccess) {
+    set_error("ma_estimate_normals: %s", cudaGetErrorString(e));
+    return 1;
+  }
+  return check_launch("ma_estimate_normals") ? 0 : 1;
+}
+
+}  // extern "C"
