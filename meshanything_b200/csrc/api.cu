@@ -435,10 +435,11 @@ int ma_decode_generate(const ma_decoder_weights* w, const float* prefix, int B, 
   }
   for (int i = 1; i < max_new && rc == 0 && !mega; i++) {
     const int ctx = PREFIX + i;                          // keys visible to this step (all rows advance together)
-    const int bucket = fast ? 0 : (ctx + 1023) / 1024;   // attention grid size class (general path)
-    const int max_keys = fast ? tmax : std::min(tmax, bucket * 1024);
+    const int bucket = (ctx + 1023) / 1024;              // attention grid size class
+    const int max_keys = std::min(tmax, bucket * 1024);
     auto enqueue = [&](cudaStream_t s) -> int {
-      if (fast) return fast_step_enqueue(w, ws.s, tmax, (__half*)kv, ws.fast, sa, !(flags & MA_GEN_NO_PDL), s);
+      if (fast)
+        return fast_step_enqueue(w, ws.s, tmax, max_keys, (__half*)kv, ws.fast, sa, !(flags & MA_GEN_NO_PDL), s);
       return enqueue_batched_step(w, ws, kv, B, T, max_keys, sa, s, tc);
     };
     if (!use_graph) {

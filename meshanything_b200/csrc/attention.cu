@@ -21,6 +21,7 @@ namespace ma {
 
 constexpr int ATT_THREADS = 256;
 constexpr int PART = 66;  // o[64], max, sum
+constexpr int ATT_MERGE_BLOCK = 2 * MA_ATTN_CHUNK * HD * 2 / (PART * 4);  // chunk partials that fit over the K / V tiles
 
 struct AttnSmem {
   __half k[MA_ATTN_CHUNK * HD];
@@ -183,17 +184,29 @@ __global__ void __launch_bounds__(ATT_THREADS) attention_kernel(AttnArgs a) {
     __syncthreads();
     if (!sm.last) return;
     __threadfence();
-    if (tid < 64) {
-      float M = -INFINITY;
+    // merge in ascending chunk order.  The partials are staged in shared memory (the K / V tiles are no longer needed)
+    // by all threads with every load in flight, so the merge costs one L2 round trip instead of a chain of them.
+    float* pst = reinterpret_cast<float*>(sm.k);
+    const bool single = nch <= ATT_MERGE_BLOCK;
+    float M = -INFINITY, L = 0.0f, O = 0.0f;
+    if (!single && tid < 64)
       for (int cc = 0; cc < nch; cc++) M = fmaxf(M, __ldcg(part + cc * PART + 64));
-      float L = 0.0f, O = 0.0f;
-      for (int cc = 0; cc < nch; cc++) {
-        const float w = ma_exp(fsub(__ldcg(part + cc * PART + 64), M));
-        L = ffma(__ldcg(part + cc * PART + 65), w, L);
-        O = ffma(__ldcg(part + cc * PART + tid), w, O);
+    for (int c0 = 0; c0 < nch; c0 += ATT_MERGE_BLOCK) {
+      const int nb = min(ATT_MERGE_BLOCK, nch - c0);
+      for (int t = tid; t < nb * PART; t += ATT_THREADS) pst[t] = __ldcg(part + (long)c0 * PART + t);
+      __syncthreads();
+      if (tid < 64) {
+        if (single)
+          for (int cc = 0; cc < nb; cc++) M = fmaxf(M, pst[cc * PART + 64]);
+        for (int cc = 0; cc < nb; cc++) {
+          const float w = ma_exp(fsub(pst[cc * PART + 64], M));
+          L = ffma(pst[cc * PART + 65], w, L);
+          O = ffma(pst[cc * PART + tid], w, O);
+        }
       }
-      a.out[(long)m * a.ldo + h * HD + tid] = __float2half_rn(__fdiv_rn(O, L));
+      __syncthreads();
     }
+    if (tid < 64) a.out[(long)m * a.ldo + h * HD + tid] = __float2half_rn(__fdiv_rn(O, L));
   } else {
     __syncthreads();
     if (tid < 64) {

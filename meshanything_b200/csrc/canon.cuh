@@ -193,16 +193,14 @@ __device__ __forceinline__ float block_sum4(float x0, float x1, float x2, float 
   return warp_tree(red, nw);
 }
 
-// LayerNorm of a row of W = 4*blockDim.x fp32 values, thread t owns elements 4t..4t+3.
-__device__ __forceinline__ void layernorm4(float* x, const float* __restrict__ gamma, const float* __restrict__ beta,
-                                           float eps, int W, float* red) {
+// LayerNorm of a row of W = 4*blockDim.x fp32 values, thread t owns elements 4t..4t+3; g / b = this thread's four
+// gamma / beta values, loaded by the caller (a PDL kernel loads them before its grid dependency resolves).
+__device__ __forceinline__ void layernorm4(float* x, const float4& g, const float4& b, float eps, int W, float* red) {
   const float inv = __fdiv_rn(1.0f, (float)W);
   float mean = fmul(block_sum4(x[0], x[1], x[2], x[3], red), inv);
   float d0 = fsub(x[0], mean), d1 = fsub(x[1], mean), d2 = fsub(x[2], mean), d3 = fsub(x[3], mean);
   float var = fmul(block_sum4(fmul(d0, d0), fmul(d1, d1), fmul(d2, d2), fmul(d3, d3), red), inv);
   float rstd = __fdiv_rn(1.0f, __fsqrt_rn(fadd(var, eps)));
-  const float4 g = *reinterpret_cast<const float4*>(gamma + 4 * threadIdx.x);
-  const float4 b = *reinterpret_cast<const float4*>(beta + 4 * threadIdx.x);
   x[0] = ffma(fmul(d0, rstd), g.x, b.x);
   x[1] = ffma(fmul(d1, rstd), g.y, b.y);
   x[2] = ffma(fmul(d2, rstd), g.z, b.z);

@@ -87,6 +87,7 @@ __global__ void __launch_bounds__(FG_THREADS) fast_gemv_kernel(FastArgs a) {
   extern __shared__ __align__(128) unsigned char smem_raw[];
   FastSmemHdr<K>& sh = *reinterpret_cast<FastSmemHdr<K>*>(smem_raw);
   __half* sw = reinterpret_cast<__half*>(smem_raw + sizeof(FastSmemHdr<K>));
+  __half* sb = sw + (size_t)a.rows_per_cta * K;  // the bias of this CTA's rows
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
   if (MODE != MODE_QKV) pdl_trigger();  // let the next kernel start streaming its weights right away
@@ -107,6 +108,17 @@ __global__ void __launch_bounds__(FG_THREADS) fast_gemv_kernel(FastArgs a) {
   if (lane == 0 && wn > 0) {
     mbar_expect_tx(&sh.bar[warp], (uint32_t)wn * K * 2);
     bulk_g2s(sw + (size_t)wr0 * K, a.W + (size_t)(row0 + wr0) * K, (uint32_t)wn * K * 2, &sh.bar[warp]);
+  }
+  // the other step-independent operands (bias, LayerNorm gamma / beta, the condition embedding) are loaded here too:
+  // read after the wait they would each add a DRAM round trip, queued behind the weight streams, to the token's chain
+  if (a.bias)
+    for (int i = tid; i < nrows; i += FG_THREADS) sb[i] = a.bias[row0 + i];
+  float4 ln_g, ln_b, cond;
+  if (MODE == MODE_QKV && a.embed) {
+    cond = *reinterpret_cast<const float4*>(a.cond + HID + 4 * tid);
+  } else if (MODE == MODE_QKV || MODE == MODE_FC1 || MODE == MODE_LM) {
+    ln_g = *reinterpret_cast<const float4*>(a.gamma + 4 * tid);
+    ln_b = *reinterpret_cast<const float4*>(a.beta + 4 * tid);
   }
 
   pdl_wait();  // everything below may read what earlier kernels wrote
@@ -132,7 +144,7 @@ __global__ void __launch_bounds__(FG_THREADS) fast_gemv_kernel(FastArgs a) {
         fidx = r + 3;
       }
       const float4 F = *reinterpret_cast<const float4*>(a.tok_pos + (long)fidx * HID + 4 * tid);
-      const float4 C = *reinterpret_cast<const float4*>(a.cond + HID + 4 * tid);
+      const float4 C = cond;
       const float4 P = *reinterpret_cast<const float4*>(a.pos_table + (long)(pos + 2) * HID + 4 * tid);
       v[0] = fadd(fadd(fadd(X.x, F.x), C.x), P.x);
       v[1] = fadd(fadd(fadd(X.y, F.y), C.y), P.y);
@@ -144,7 +156,7 @@ __global__ void __launch_bounds__(FG_THREADS) fast_gemv_kernel(FastArgs a) {
       const __half2* h = reinterpret_cast<const __half2*>(&u);
       const float2 p0 = __half22float2(h[0]), p1 = __half22float2(h[1]);
       v[0] = fadd(hv.x, p0.x); v[1] = fadd(hv.y, p0.y); v[2] = fadd(hv.z, p1.x); v[3] = fadd(hv.w, p1.y);
-      layernorm4(v, a.gamma, a.beta, MA_LN_EPS, HID, sh.red);
+      layernorm4(v, ln_g, ln_b, MA_LN_EPS, HID, sh.red);
     }
     if (blockIdx.x == 0 && a.hres_out)
       *reinterpret_cast<float4*>(a.hres_out + 4 * tid) = make_float4(v[0], v[1], v[2], v[3]);
@@ -196,7 +208,7 @@ __global__ void __launch_bounds__(FG_THREADS) fast_gemv_kernel(FastArgs a) {
       const float sum = warp_sum(acc[i]);
       const int n = row0 + wr0 + r0 + i;
       if (r0 + i < wn && lane == 0) {
-        const float bf = a.bias ? __half2float(a.bias[n]) : 0.0f;
+        const float bf = a.bias ? __half2float(sb[wr0 + r0 + i]) : 0.0f;
         __half h = __float2half_rn(fadd(sum, bf));
         if (MODE == MODE_FC1 && __half2float(h) < 0.0f) h = __float2half_rn(0.0f);
         if (MODE == MODE_QKV) {
@@ -292,7 +304,7 @@ size_t fast_workspace_bytes() {
 
 template <int K, int MODE>
 static int launch_fast(const FastArgs& a, int grid, bool pdl, cudaStream_t st) {
-  const size_t smem = sizeof(FastSmemHdr<K>) + (size_t)a.rows_per_cta * K * 2;
+  const size_t smem = sizeof(FastSmemHdr<K>) + (size_t)a.rows_per_cta * K * 2 + (((size_t)a.rows_per_cta * 2 + 15) & ~(size_t)15);
   static size_t attr_set = 0;
   if (smem > attr_set) {
     cudaFuncSetAttribute(fast_gemv_kernel<K, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -313,7 +325,7 @@ static int launch_fast(const FastArgs& a, int grid, bool pdl, cudaStream_t st) {
   return check_launch("fast_gemv_kernel") ? 0 : 1;
 }
 
-int fast_step_enqueue(const ma_decoder_weights* w, SeqState s, int tmax, __half* kv, void* fast_ws,
+int fast_step_enqueue(const ma_decoder_weights* w, SeqState s, int tmax, int max_keys, __half* kv, void* fast_ws,
                       const SampleArgs& sa, bool pdl, cudaStream_t st) {
   if (!g_sms) {
     int dev = 0;
@@ -347,7 +359,7 @@ int fast_step_enqueue(const ma_decoder_weights* w, SeqState s, int tmax, __half*
       a.out16 = ws->q; a.kc = kc; a.vc = vc;
       if (launch_fast<HID, MODE_QKV>(a, grid, pdl, st)) return 1;
     }
-    if (launch_attention_ex(ws->q, HID, kc, vc, T, NHEAD, 1, nullptr, &ws->nkeys, tmax, 1, 0.125f, ws->attn16, HID,
+    if (launch_attention_ex(ws->q, HID, kc, vc, T, NHEAD, 1, nullptr, &ws->nkeys, max_keys, 1, 0.125f, ws->attn16, HID,
                             ws->attn_scratch, 1, pdl, st)) return 1;
     {  // out_proj
       FastArgs a = base;

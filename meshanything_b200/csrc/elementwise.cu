@@ -31,7 +31,8 @@ __global__ void layernorm_kernel(const float* __restrict__ x, const __half* __re
       v[0] = a.x; v[1] = a.y; v[2] = b.x; v[3] = b.y;
     }
   }
-  layernorm4(v, gamma, beta, eps, W, red);
+  layernorm4(v, *reinterpret_cast<const float4*>(gamma + 4 * t), *reinterpret_cast<const float4*>(beta + 4 * t), eps, W,
+             red);
   if (out32) *reinterpret_cast<float4*>(out32 + row * W + 4 * t) = make_float4(v[0], v[1], v[2], v[3]);
   if (out16) {
     __half2 h0 = __floats2half2_rn(v[0], v[1]), h1 = __floats2half2_rn(v[2], v[3]);

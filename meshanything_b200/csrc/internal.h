@@ -99,7 +99,8 @@ int launch_fill_i32(int32_t* p, int v, long n, cudaStream_t st);
 // decode_fast.cu (batch-1 fused GEMV path)
 int* fast_nkeys_ptr(void* fast_ws);
 size_t fast_workspace_bytes();
-int fast_step_enqueue(const ma_decoder_weights* w, SeqState s, int tmax, __half* kv, void* fast_ws,
+// max_keys: the attention grid covers this many keys; no step of the launch may see more
+int fast_step_enqueue(const ma_decoder_weights* w, SeqState s, int tmax, int max_keys, __half* kv, void* fast_ws,
                       const SampleArgs& sa, bool pdl, cudaStream_t st);
 
 
