@@ -341,6 +341,28 @@ int ma_estimate_normals(const float* xyz, int n, int k, float* normals_out, int3
 void ma_estimate_normals_set_events(void* const* events);
 int ma_estimate_normals_last_rounds(void);
 
+/* ---- outlier removal of a point cloud (`--remove_outliers`; csrc/outliers.cu) ------------------------------------
+ * xyz fp32 [n][3], finite, already in the output frame -> the points DESIGN.md section 1.3 keeps: with the exact kNN
+ * of section 1.2, d_i = the fp64 mean of the fp32 sqrt(d^2) of point i's k neighbours; statistical inlier iff
+ * d_i <= mu + std_ratio sigma (mu, sigma over all points, fixed-order fp64 sums); then the connected components of the
+ * kNN graph among the inliers, a component kept iff size >= min_component * inliers or it is the largest (lowest
+ * label on ties); min_component = 0 keeps every inlier.
+ * Device outputs: keep_out uint8 [n] (1 = kept), kept_idx_out int64 [n] (the first *n_kept_out entries: the kept
+ * indices, ascending), n_kept_out int64 [1], stats_out fp64 [8] = (mu, sigma, threshold, statistical inliers,
+ * components (0 when the stage is off), components dropped, kept points, connectivity rounds).  Optional (NULL: not
+ * written): mean_dist_out fp64 [n] (d_i), knn_out int32 [n][k] (rank order).
+ * 1 <= k <= 64, k < n <= 2^24, std_ratio finite, min_component finite and >= 0.  ws:
+ * ma_remove_outliers_workspace_bytes(n, k) bytes (0 for shapes out of range).  Synchronises the stream once for the
+ * grid's extent (24 bytes) and once per connectivity round (4 bytes).  Two calls give identical bits, except the
+ * round count, which depends on the schedule. */
+size_t ma_remove_outliers_workspace_bytes(int n, int k);
+int ma_remove_outliers(const float* xyz, int n, int k, double std_ratio, double min_component, uint8_t* keep_out,
+                       int64_t* kept_idx_out, int64_t* n_kept_out, double* mean_dist_out, int32_t* knn_out,
+                       double* stats_out, void* ws, void* stream);
+/* Measurement hook (tools/bench_outliers.py): events = 5 cudaEvent_t recorded on the stream of every following call at
+ * its start and after the grid build, the kNN, the statistical stage and the component stage (NULL: off). */
+void ma_remove_outliers_set_events(void* const* events);
+
 /* number of kernels launched by the library since load (bench.py's gpu_launches) */
 unsigned long long ma_launch_count(void);
 

@@ -2,6 +2,7 @@
 
     python main.py --input_type pc_normal --input_path pc_examples/mouse.npy --out_dir out [--sampling]
     python main.py --input_type pc --input_path scan.npy       # bare (N, 3) cloud: normals estimated on the GPU
+    python main.py --input_type pc --input_path scan.npy --remove_outliers   # drop stray points / floaters first
     torchrun --nproc-per-node 8 main.py --input_type pc_normal --input_dir pcs --batchsize_per_gpu 64
 
 Differences forced by the environment: no accelerate / hf_hub (there is no network) -- one process per
@@ -21,25 +22,45 @@ from MeshAnything.models.meshanything import MeshAnything
 from mesh_to_pc import load_mesh, process_mesh_to_pc
 
 
-def _subsample_points(path, n_points=4096):
+def _remove_outliers(xyz, path, outliers, n_points=4096):
+    """`--remove_outliers`: the indices of the points of xyz [N, 3] that DESIGN.md section 1.3 keeps (on the GPU,
+    meshanything_b200.outliers), with one line of counts per input."""
+    from meshanything_b200.outliers import remove_outliers
+    idx, st = remove_outliers(xyz, **outliers)
+    print(f"{_uid_of(path)}: removed {st.removed_statistical} of {st.n_points} points by neighbour distance, "
+          f"{st.removed_components} more in {st.components_dropped} of {st.components} components; {st.kept} kept")
+    if st.kept < n_points:
+        raise ValueError(f"{path}: {st.kept} points remain after outlier removal ({st.removed_statistical} removed by "
+                         f"neighbour distance, {st.removed_components} in {st.components_dropped} small components), "
+                         f"fewer than the {n_points} the model takes")
+    return idx.cpu().numpy()
+
+
+def _subsample_points(path, n_points=4096, outliers=None):
     """`--input_type pc_normal`: an .npy of >= 4096 (xyz, normal) rows; a random 4096-subset without replacement
-    (global numpy RNG, seeded by --seed as the reference does through accelerate.set_seed)."""
+    (global numpy RNG, seeded by --seed as the reference does through accelerate.set_seed).  With `outliers` (the
+    keyword arguments of meshanything_b200.outliers.remove_outliers) the rows are first cleaned by their xyz."""
     cloud = np.load(path)
+    if outliers is not None:
+        cloud = cloud[_remove_outliers(cloud[:, :3], path, outliers, n_points)]
     assert cloud.shape[0] >= n_points, "input pc_normal should have at least 4096 points"
     keep = np.random.choice(cloud.shape[0], n_points, replace=False)
     return cloud[keep]
 
 
-def _points_with_normals(path, n_points=4096, k=16):
+def _points_with_normals(path, n_points=4096, k=16, outliers=None):
     """`--input_type pc`: a bare cloud (.npy (N, 3) or vertex-only .ply) of >= 4096 points.  Normals are estimated on
     the GPU from all N points (meshanything_b200.normals), then the same random 4096-subset as `pc_normal` is drawn: the
-    xyz-only copy of a file selects the points the file with normals selects under the same seed."""
+    xyz-only copy of a file selects the points the file with normals selects under the same seed.  With `outliers`
+    the cloud is cleaned first, and normals and subset come from the kept points."""
     from mesh_to_pc import load_points
     from meshanything_b200.normals import estimate_normals
     xyz = load_points(path)
     if not np.issubdtype(xyz.dtype, np.floating):
         xyz = xyz.astype(np.float64)
     assert xyz.shape[0] >= n_points, "input pc_normal should have at least 4096 points"
+    if outliers is not None:
+        xyz = xyz[_remove_outliers(xyz, path, outliers, n_points)]
     normals = estimate_normals(xyz, k).cpu().numpy()
     keep = np.random.choice(xyz.shape[0], n_points, replace=False)
     return np.concatenate([xyz[keep], normals[keep].astype(xyz.dtype)], axis=1)
@@ -49,15 +70,23 @@ def _uid_of(path):
     return path.split('/')[-1].split('.')[0]
 
 
+_NO_MESH_OUTLIERS = ("--remove_outliers applies to point-cloud input (--input_type pc or pc_normal): the points of a "
+                     "mesh are sampled from its surface and have no outliers")
+
+
 class Dataset:
     """Same contract as the reference's Dataset (main.py:15-58): items are {'pc_normal': fp16 (4096, 6), 'uid': str},
-    coordinates centred on the bounding box and scaled to max |x| = 0.9995, unit normals asserted."""
+    coordinates centred on the bounding box and scaled to max |x| = 0.9995, unit normals asserted.  `outliers` (point
+    clouds only): None, or the keyword arguments of meshanything_b200.outliers.remove_outliers, to clean every cloud
+    before normals and subset."""
 
-    def __init__(self, input_type, input_list, mc=False):
+    def __init__(self, input_type, input_list, mc=False, outliers=None):
+        if outliers is not None and input_type not in ('pc', 'pc_normal'):
+            raise ValueError(_NO_MESH_OUTLIERS)
         if input_type == 'pc_normal':
-            clouds = [_subsample_points(p) for p in input_list]
+            clouds = [_subsample_points(p, outliers=outliers) for p in input_list]
         elif input_type == 'pc':
-            clouds = [_points_with_normals(p) for p in input_list]
+            clouds = [_points_with_normals(p, outliers=outliers) for p in input_list]
         elif input_type == 'mesh':
             if mc:
                 print("First Marching Cubes and then sample point cloud, need several minutes...")
@@ -99,7 +128,21 @@ def get_args():
     # not in the reference: sample N meshes of every shape in one batch and keep the one closest to the input cloud
     # (Chamfer distance on the GPU; MeshAnything.forward_candidates) instead of re-rolling --seed by hand
     parser.add_argument('--num_samples', default=1, type=int)
+    # not in the reference: drop stray points and small floating clusters of a scan before normals and normalisation
+    # (DESIGN.md section 1.3; meshanything_b200.outliers); the parameters follow Open3D's remove_statistical_outlier
+    parser.add_argument('--remove_outliers', default=False, action="store_true")
+    parser.add_argument('--outlier_neighbors', default=16, type=int)
+    parser.add_argument('--outlier_std_ratio', default=2.0, type=float)
+    parser.add_argument('--outlier_min_component', default=0.01, type=float)
     return parser.parse_args()
+
+
+def outlier_options(args):
+    """The `outliers` argument of Dataset from the command line: None without --remove_outliers."""
+    if not args.remove_outliers:
+        return None
+    return {'k': args.outlier_neighbors, 'std_ratio': args.outlier_std_ratio,
+            'min_component': args.outlier_min_component}
 
 
 def check_args(args):
@@ -110,6 +153,14 @@ def check_args(args):
     if args.num_samples > 1 and args.continuous_batching:
         raise ValueError("--num_samples > 1 does not run with --continuous_batching: best-of-N scores the candidates "
                          "of a padded batch together")
+    if args.remove_outliers:
+        if args.input_type == 'mesh':
+            raise ValueError(_NO_MESH_OUTLIERS)
+        if not 1 <= args.outlier_neighbors <= 64:
+            raise ValueError(f"--outlier_neighbors must be in 1..64, got {args.outlier_neighbors}")
+        if not (np.isfinite(args.outlier_std_ratio) and np.isfinite(args.outlier_min_component)
+                and args.outlier_min_component >= 0):
+            raise ValueError("--outlier_std_ratio must be finite and --outlier_min_component finite and >= 0")
 
 
 def load_model(args, device=None):
@@ -233,7 +284,7 @@ if __name__ == "__main__":
         raise ValueError("input_dir or input_path must be provided.")
     np.random.seed(args.seed)
     torch.manual_seed(args.seed)
-    dataset = Dataset(args.input_type, input_list, args.mc)
+    dataset = Dataset(args.input_type, input_list, args.mc, outliers=outlier_options(args))
 
     bs = args.batchsize_per_gpu
     batches = [list(range(i, min(i + bs, len(dataset)))) for i in range(0, len(dataset), bs)]

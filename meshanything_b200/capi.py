@@ -6,6 +6,7 @@ PyTorch fallback: if the shared object cannot be loaded every call raises.
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 from typing import Optional
 
@@ -49,6 +50,7 @@ EXPORTS = [
     "ma_mesh_score_workspace_bytes", "ma_mesh_score",
     "ma_estimate_normals_workspace_bytes", "ma_estimate_normals", "ma_estimate_normals_set_events",
     "ma_estimate_normals_last_rounds",
+    "ma_remove_outliers_workspace_bytes", "ma_remove_outliers", "ma_remove_outliers_set_events",
 ]
 
 
@@ -132,6 +134,12 @@ def lib():
     L.ma_estimate_normals_set_events.restype = None
     L.ma_estimate_normals_last_rounds.argtypes = []
     L.ma_estimate_normals_last_rounds.restype = C.c_int
+    L.ma_remove_outliers_workspace_bytes.argtypes = [C.c_int, C.c_int]
+    L.ma_remove_outliers_workspace_bytes.restype = C.c_size_t
+    L.ma_remove_outliers.argtypes = [_vp, C.c_int, C.c_int, C.c_double, C.c_double, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                     _vp]
+    L.ma_remove_outliers_set_events.argtypes = [_vp]
+    L.ma_remove_outliers_set_events.restype = None
     L.ma_linear_tc_f16.argtypes = [_vp, _vp, _vp, C.c_int, _vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _vp]
     L.ma_set_tensor_cores.argtypes = [C.c_int]
     L.ma_tensor_core_linear_counts.argtypes = [C.POINTER(C.c_ulonglong), C.POINTER(C.c_ulonglong)]
@@ -290,6 +298,45 @@ def estimate_normals(points: torch.Tensor, k: int = 16, want_terms: bool = False
     check(lib().ma_estimate_normals(ptr(p), n, k, ptr(out), ptr(knn), ptr(uno), ptr(ws), stream_ptr()),
           "ma_estimate_normals")
     return (out, knn, uno) if want_terms else out
+
+
+def remove_outliers(points: torch.Tensor, k: int = 16, std_ratio: float = 2.0, min_component: float = 0.01,
+                    want_terms: bool = False):
+    """Outlier removal of a cloud (ma_remove_outliers; outliers.remove_outliers adds the frame map).
+
+    points fp32 [N, 3], finite, already in the output frame; 1 <= k <= 64, k < N <= 2^24.  Returns (kept indices int64
+    [n_kept] ascending, keep mask bool [N], stats fp64 [8] on the host: mu, sigma, threshold, statistical inliers,
+    components, components dropped, kept points, connectivity rounds); with want_terms also (mean neighbour distance
+    fp64 [N], kNN int32 [N, k] in rank order).  Reads the stats back (synchronises)."""
+    _need_cuda(points)
+    p = points.to(torch.float32).contiguous()
+    if p.dim() != 2 or p.shape[1] != 3:
+        raise ValueError("remove_outliers: points [N, 3]")
+    n = p.shape[0]
+    if not 1 <= k <= 64:
+        raise ValueError(f"remove_outliers: 1 <= k <= 64, got k = {k}")
+    if not k < n <= 1 << 24:
+        raise ValueError(f"remove_outliers: k < N <= 2^24, got N = {n}, k = {k}")
+    if not math.isfinite(std_ratio):
+        raise ValueError(f"remove_outliers: std_ratio must be finite, got {std_ratio}")
+    if not (math.isfinite(min_component) and min_component >= 0):
+        raise ValueError(f"remove_outliers: min_component must be finite and >= 0, got {min_component}")
+    if not bool(torch.isfinite(p).all()):
+        raise ValueError("remove_outliers: non-finite coordinates")
+    dev = p.device
+    ws = torch.empty(lib().ma_remove_outliers_workspace_bytes(n, k), dtype=torch.uint8, device=dev)
+    keep = torch.empty((n,), dtype=torch.uint8, device=dev)
+    idx = torch.empty((n,), dtype=torch.int64, device=dev)
+    n_kept = torch.empty((1,), dtype=torch.int64, device=dev)
+    stats = torch.empty((8,), dtype=torch.float64, device=dev)
+    mean = torch.empty((n,), dtype=torch.float64, device=dev) if want_terms else None
+    knn = torch.empty((n, k), dtype=torch.int32, device=dev) if want_terms else None
+    check(lib().ma_remove_outliers(ptr(p), n, k, C.c_double(std_ratio), C.c_double(min_component), ptr(keep), ptr(idx),
+                                   ptr(n_kept), ptr(mean), ptr(knn), ptr(stats), ptr(ws), stream_ptr()),
+          "ma_remove_outliers")
+    st = stats.cpu().numpy()
+    out = (idx[:int(st[6])], keep.bool(), st)
+    return (*out, mean, knn) if want_terms else out
 
 
 def tensor_core_linear_counts():

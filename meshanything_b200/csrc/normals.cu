@@ -1,14 +1,10 @@
 // normals.cu -- oriented normals of a bare point cloud for `--input_type pc` (DESIGN.md section 1.2 defines them).
 //
 // The points arrive already in the output frame (p' = (p - c) / L, metrics.to_output_frame), fp32 [N][3].
-//   (a) grid      normals_cell_kernel counts the points per cell of a G^3 grid over [-0.5, 0.5]^3, a CUB exclusive
-//                 scan gives the cell starts, normals_scatter_kernel writes the points in cell order (float4: xyz and
-//                 the original index).  The order inside a cell is whatever the atomics give: nothing depends on it.
-//   (b) kNN       normals_knn_kernel, one thread per point: shells of cells by Chebyshev radius r = 0, 1, ... around
-//                 the query's cell, every candidate keyed by (fp32 d^2 bits << 32 | index), the k smallest keys kept
-//                 sorted in shared memory.  After shell r it stops when the k-th key's d^2 is below a lower bound of
-//                 the distance to every cell outside the shells (shrunk by a margin far above fp32 rounding), or when
-//                 no cell is left.  The grid size therefore only changes the speed: the result is the exact kNN.
+//   (a) grid      knn_cell_kernel / knn_scatter_kernel (knn_grid.cuh) sort the points into a G^3 grid over
+//                 [-0.5, 0.5]^3 (lo = -0.5, scale = G), a CUB exclusive scan giving the cell starts.
+//   (b) kNN       knn_grid_kernel (knn_grid.cuh), one thread per point, shells of cells until the k-th key's d^2 is
+//                 below the bound of the next shell, without a shell budget: the exact kNN.
 //   (c) PCA       normals_pca_kernel, one thread per point: fp64 centroid and covariance of the point and its
 //                 neighbours in rank order, sequential sums of explicit __d*_rn operations, then kNmSweeps cyclic
 //                 Jacobi sweeps; the eigenvector of the smallest diagonal entry, normalised in fp64, rounded to fp32.
@@ -27,120 +23,23 @@
 
 #include "canon.cuh"
 #include "internal.h"
+#include "knn_grid.cuh"
 
 namespace ma {
 
 constexpr int kNmThreads = 256;
-constexpr int kNmKnnThreads = 64;   // kNN threads per CTA: k x 64 x 8 B of shared memory for the top-k lists
 constexpr int kNmSweeps = 5;        // Jacobi sweeps: 4 reach 4e-15 rad against LAPACK on separated spectra, 1 spare
-constexpr int kNmMaxK = 64;
 constexpr int kNmMaxN = 1 << 24;    // vertex words hold the root in 31 bits; the index part of a kNN key in 32
-constexpr int kNmMaxG = 256;
 constexpr int kNmMaxRounds = 64;    // Boruvka at least halves the components with an outgoing edge per round
 
-// grid cells per axis: about 4 k points per occupied cell of a surface, so that radius 1 mostly suffices
-static int nm_grid(int n, int k) {
-  const int g = (int)ceil(0.5 * sqrt((double)n / (double)k));
-  return std::max(1, std::min(kNmMaxG, g));
-}
-
-__device__ __forceinline__ int nm_cell1(float x, int G) {
-  const int c = (int)floorf(__fmul_rn(__fadd_rn(x, 0.5f), (float)G));
-  return min(max(c, 0), G - 1);
+// the grid over the whole frame [-0.5, 0.5]^3
+static KnnGrid nm_grid(int n, int k) {
+  const int G = knn_grid_size(n, k);
+  return KnnGrid{{-0.5f, -0.5f, -0.5f}, (float)G, 1.0f / (float)G, G};
 }
 
 __device__ __forceinline__ float nm_dot(float ax, float ay, float az, float bx, float by, float bz) {
   return __fadd_rn(__fadd_rn(__fmul_rn(ax, bx), __fmul_rn(ay, by)), __fmul_rn(az, bz));
-}
-
-// ---------------------------------------------------------------- (a) grid
-
-__global__ void normals_cell_kernel(const float* __restrict__ xyz, int n, int G, uint32_t* __restrict__ cell,
-                                    uint32_t* __restrict__ count) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const float* p = xyz + 3 * (size_t)i;
-  const uint32_t c = ((uint32_t)nm_cell1(p[0], G) * G + nm_cell1(p[1], G)) * G + nm_cell1(p[2], G);
-  cell[i] = c;
-  atomicAdd(count + c, 1u);
-}
-
-// count[c] is used up as a cursor: the point takes slot start[c] + (atomicSub's old value - 1)
-__global__ void normals_scatter_kernel(const float* __restrict__ xyz, int n, const uint32_t* __restrict__ cell,
-                                       const uint32_t* __restrict__ start, uint32_t* __restrict__ count,
-                                       float4* __restrict__ sorted) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  const uint32_t c = cell[i];
-  const uint32_t slot = start[c] + atomicSub(count + c, 1u) - 1u;
-  const float* p = xyz + 3 * (size_t)i;
-  sorted[slot] = make_float4(p[0], p[1], p[2], __int_as_float(i));
-}
-
-// ---------------------------------------------------------------- (b) exact kNN
-
-__global__ void __launch_bounds__(kNmKnnThreads) normals_knn_kernel(const float4* __restrict__ sorted,
-                                                                    const uint32_t* __restrict__ start, int n, int k,
-                                                                    int G, int32_t* __restrict__ knn) {
-  extern __shared__ unsigned long long nm_top[];  // [k][kNmKnnThreads]: entry e of thread t at e * 64 + t
-  const int s = blockIdx.x * kNmKnnThreads + threadIdx.x;
-  if (s >= n) return;
-  unsigned long long* top = nm_top + threadIdx.x;
-  const float4 q = sorted[s];
-  const int self = __float_as_int(q.w);
-  const int cx = nm_cell1(q.x, G), cy = nm_cell1(q.y, G), cz = nm_cell1(q.z, G);
-  const float inv = 1.0f / (float)G;
-  int m = 0;
-  for (int r = 0;; r++) {
-    for (int dx = -r; dx <= r; dx++) {
-      const int x = cx + dx;
-      if (x < 0 || x >= G) continue;
-      for (int dy = -r; dy <= r; dy++) {
-        const int y = cy + dy;
-        if (y < 0 || y >= G) continue;
-        // the shell of radius r: whole z columns on its x / y faces, only dz = -r and +r inside them
-        const int step = (r == 0 || dx == -r || dx == r || dy == -r || dy == r) ? 1 : 2 * r;
-        for (int dz = -r; dz <= r; dz += step) {
-          const int z = cz + dz;
-          if (z < 0 || z >= G) continue;
-          const uint32_t c = ((uint32_t)x * G + y) * G + z;
-          const uint32_t e1 = start[c + 1];
-          for (uint32_t t = start[c]; t < e1; t++) {
-            const float4 p = sorted[t];
-            const int j = __float_as_int(p.w);
-            if (j == self) continue;
-            const float ex = __fsub_rn(q.x, p.x), ey = __fsub_rn(q.y, p.y), ez = __fsub_rn(q.z, p.z);
-            const float d2 = __fadd_rn(__fadd_rn(__fmul_rn(ex, ex), __fmul_rn(ey, ey)), __fmul_rn(ez, ez));
-            const unsigned long long key = ((unsigned long long)__float_as_uint(d2) << 32) | (uint32_t)j;
-            if (m == k && key >= top[(size_t)(k - 1) * kNmKnnThreads]) continue;
-            int e = m < k ? m++ : k - 1;
-            while (e > 0 && top[(size_t)(e - 1) * kNmKnnThreads] > key) {
-              top[(size_t)e * kNmKnnThreads] = top[(size_t)(e - 1) * kNmKnnThreads];
-              e--;
-            }
-            top[(size_t)e * kNmKnnThreads] = key;
-          }
-        }
-      }
-    }
-    // lower bound of the distance from q to any cell outside the cube [c - r, c + r]^3 (only the sides that have cells)
-    float b = INFINITY;
-    if (cx - r > 0) b = fminf(b, q.x - ((float)(cx - r) * inv - 0.5f));
-    if (cx + r < G - 1) b = fminf(b, ((float)(cx + r + 1) * inv - 0.5f) - q.x);
-    if (cy - r > 0) b = fminf(b, q.y - ((float)(cy - r) * inv - 0.5f));
-    if (cy + r < G - 1) b = fminf(b, ((float)(cy + r + 1) * inv - 0.5f) - q.y);
-    if (cz - r > 0) b = fminf(b, q.z - ((float)(cz - r) * inv - 0.5f));
-    if (cz + r < G - 1) b = fminf(b, ((float)(cz + r + 1) * inv - 0.5f) - q.z);
-    if (b == INFINITY) break;  // every cell has been searched
-    if (m == k) {
-      // margin: a point can sit ~1e-7 outside its cell after fp32 rounding, and d^2 carries a few ulps of error; a
-      // strict < because an unseen point at the same d^2 with a lower index would still rank first
-      const float bs = fmaxf(b - 1e-6f, 0.0f);
-      if (__uint_as_float((uint32_t)(top[(size_t)(k - 1) * kNmKnnThreads] >> 32)) < bs * bs * (1.0f - 1e-5f)) break;
-    }
-  }
-  int32_t* out = knn + (size_t)self * k;
-  for (int e = 0; e < k; e++) out[e] = (int32_t)(uint32_t)top[(size_t)e * kNmKnnThreads];
 }
 
 // ---------------------------------------------------------------- (c) PCA + Jacobi
@@ -348,7 +247,7 @@ __global__ void normals_apply_kernel(const float* __restrict__ xyz, const float*
 // ---------------------------------------------------------------- workspace
 
 static size_t nm_align(size_t b) { return (b + 255) & ~(size_t)255; }
-static bool nm_shape_ok(int n, int k) { return k >= 1 && k <= kNmMaxK && n > k && n <= kNmMaxN; }
+static bool nm_shape_ok(int n, int k) { return k >= 1 && k <= kKnnMaxK && n > k && n <= kNmMaxN; }
 
 static size_t nm_scan_bytes(size_t cells) {
   size_t bytes = 0;
@@ -361,7 +260,7 @@ struct NmLayout {
 };
 
 static NmLayout nm_layout(int n, int k) {
-  const int G = nm_grid(n, k);
+  const int G = nm_grid(n, k).G;
   const size_t cells = (size_t)G * G * G, nk = (size_t)n * k;
   NmLayout L;
   size_t o = 0;
@@ -415,7 +314,7 @@ int ma_estimate_normals_last_rounds(void) { return g_nm_rounds; }
 int ma_estimate_normals(const float* xyz, int n, int k, float* normals_out, int32_t* knn_out, float* unoriented_out,
                         void* ws, void* stream) {
   if (!xyz || !normals_out || !ws || !nm_shape_ok(n, k)) {
-    set_error("ma_estimate_normals: bad arguments (1 <= k <= %d, k < n <= 2^24)", kNmMaxK);
+    set_error("ma_estimate_normals: bad arguments (1 <= k <= %d, k < n <= 2^24)", kKnnMaxK);
     return 1;
   }
   cudaStream_t st = (cudaStream_t)stream;
@@ -433,7 +332,8 @@ int ma_estimate_normals(const float* xyz, int n, int k, float* normals_out, int3
   auto* best1 = reinterpret_cast<unsigned long long*>(base + L.best1);
   auto* best2 = reinterpret_cast<uint32_t*>(base + L.best2);
   auto* hooks = reinterpret_cast<int*>(base + L.hooks);
-  const int G = nm_grid(n, k);
+  const KnnGrid grid = nm_grid(n, k);
+  const int G = grid.G;
   const size_t cells = (size_t)G * G * G, nk = (size_t)n * k;
 
   nm_mark(0, st);
@@ -442,14 +342,15 @@ int ma_estimate_normals(const float* xyz, int n, int k, float* normals_out, int3
     set_error("ma_estimate_normals: %s", cudaGetErrorString(e));
     return 1;
   }
-  normals_cell_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(xyz, n, G, cell, count);
+  knn_cell_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(xyz, n, grid, cell, count);
   size_t scan_bytes = nm_scan_bytes(cells);
   e = cub::DeviceScan::ExclusiveSum(base + L.scan, scan_bytes, count, start, (int)(cells + 1), st);
-  normals_scatter_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(xyz, n, cell, start, count, sorted);
+  knn_scatter_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(xyz, n, cell, start, count, sorted);
   count_launch(3);
   nm_mark(1, st);
-  normals_knn_kernel<<<(n + kNmKnnThreads - 1) / kNmKnnThreads, kNmKnnThreads,
-                       (size_t)k * kNmKnnThreads * sizeof(unsigned long long), st>>>(sorted, start, n, k, G, knn);
+  knn_grid_kernel<false><<<(n + kKnnThreads - 1) / kKnnThreads, kKnnThreads,
+                           (size_t)k * kKnnThreads * sizeof(unsigned long long), st>>>(sorted, start, n, k, grid, 0,
+                                                                                       nullptr, nullptr, knn, nullptr);
   nm_mark(2, st);
   normals_pca_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(xyz, knn, n, k, uno);
   nm_mark(3, st);
