@@ -214,9 +214,11 @@ __device__ __forceinline__ bool better(float v, int i, float bv, int bi) { retur
 constexpr int SAMPLE_THREADS = 256;
 constexpr int KEEP_MAX = 256;  // capacity of the kept set (top_k plus ties at the threshold)
 
-// order-preserving 16-bit key of an fp16 value: larger value <=> larger key (-0 < +0, irrelevant here)
+// order-preserving 16-bit key of an fp16 value: larger value <=> larger key, equal values <=> equal keys.  -0 takes
+// +0's key: TopKLogitsWarper's `scores < kth` keeps every zero when the k-th largest value is a zero of either sign.
 __device__ __forceinline__ unsigned key16(__half h) {
-  const unsigned u = __half_as_ushort(h);
+  unsigned u = __half_as_ushort(h);
+  if (u == 0x8000u) u = 0u;
   return (u & 0x8000u) ? (~u & 0xffffu) : (u | 0x8000u);
 }
 

@@ -10,7 +10,8 @@ Two layers:
   * `SlotEngine` -- that interface on the GPU over the C ABI (`ma_decode_slots_*`, include/meshanything_b200.h).
 
 Rows never interact and the kernels are batch-invariant, so every sequence gets the ids a solo
-`Generator.generate` gives it (greedy; with sampling the Philox stream is keyed by the slot a shape lands in).
+`Generator.generate` gives it (greedy; with sampling the Philox stream is keyed by the shape's index in the queue,
+whatever slot it lands in).
 """
 from __future__ import annotations
 

@@ -3,15 +3,16 @@
 `OracleDecoder.generate` restates what `MeshAnything.forward` asks of HF `generate()`
 (/root/reference/MeshAnything/models/meshanything.py:144-162) for transformers==4.39.3
 `GenerationMixin._greedy_search`: step 0 feeds `inputs_embeds`, later steps feed only the last id;
-greedy = argmax of the fp16 logits (lowest index on ties); a finished row emits pad; stop when every
-row has produced eos or after `max_new_tokens`.
+greedy = argmax of the fp16 logits (lowest index on ties), or any other pick the caller passes (the sampler
+restatement of tests/sampler_oracle.py); a finished row emits pad; stop when every row has produced eos or after
+`max_new_tokens`.
 """
 from __future__ import annotations
 
 import ctypes as C
 import os
 import subprocess
-from typing import Dict, List, Optional, Tuple
+from typing import Callable, Dict, List, Optional, Tuple
 
 import numpy as np
 import torch
@@ -49,6 +50,8 @@ def lib():
         L.orc_attention.argtypes = [u16p, u16p, u16p, i32p, C.c_int, C.c_int, C.c_long, u16p]
         L.orc_exp.argtypes = [C.c_float]
         L.orc_exp.restype = C.c_float
+        L.orc_exp_n.argtypes = [f32p, C.c_int, f32p]
+        L.orc_exp_n.restype = None
         L.orc_set_threads.argtypes = [C.c_int]
         L.orc_set_threads.restype = None
         L.orc_max_threads.restype = C.c_int
@@ -198,11 +201,13 @@ class OracleDecoder:
         return torch.from_numpy(out.view(np.float16).copy())
 
     def generate(self, prefix: torch.Tensor, max_new_tokens: int, eos_id: int = 1, pad_id: int = 2,
-                 forced: Optional[List[int]] = None, keep_logits: bool = False):
+                 forced: Optional[List[int]] = None, keep_logits: bool = False,
+                 pick: Optional[Callable[[torch.Tensor, int], int]] = None):
         """Greedy generate() for ONE sequence.  Returns (ids list, logits list).
 
         `forced`: teacher forcing -- feed these ids instead of the argmax (logits are still returned),
         used to compare logits along a sequence produced elsewhere.
+        `pick(logits, step) -> id`: replaces the argmax, e.g. the sampler restatement of tests/sampler_oracle.py.
         """
         self.reset()
         ids: List[int] = []
@@ -212,10 +217,10 @@ class OracleDecoder:
         for i in range(max_new_tokens):
             if keep_logits:
                 all_logits.append(logits)
-            nxt = int(torch.argmax(logits.float()).item())  # torch CPU argmax: first max index
-            # lowest index among exact fp16 ties (float() is exact)
-            mx = logits.float().max()
-            nxt = int((logits.float() == mx).nonzero()[0].item())
+            if pick is not None:
+                nxt = int(pick(logits, i))
+            else:
+                nxt = greedy_pick(logits)   # lowest index among exact fp16 ties (float() is exact)
             if forced is not None:
                 nxt = forced[i]
             if finished:

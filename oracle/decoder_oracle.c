@@ -352,6 +352,11 @@ void orc_attention(const uint16_t *q_, const uint16_t *K_, const uint16_t *V_, c
 
 float orc_exp(float x) { return ma_exp(x); }
 
+/* y[i] = ma_exp(x[i]): the sampler restatement (tests/sampler_oracle.py) calls this once per kept set */
+void orc_exp_n(const float *x, int n, float *y) {
+  for (int i = 0; i < n; i++) y[i] = ma_exp(x[i]);
+}
+
 /* ------------------------------------------------------------------ the decoder */
 
 typedef struct {
