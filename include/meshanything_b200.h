@@ -363,6 +363,26 @@ int ma_remove_outliers(const float* xyz, int n, int k, double std_ratio, double 
  * its start and after the grid build, the kNN, the statistical stage and the component stage (NULL: off). */
 void ma_remove_outliers_set_events(void* const* events);
 
+/* ---- farthest-point subsampling of a point cloud (`--subsample fps`; csrc/subsample.cu) ---------------------------
+ * xyz fp32 [n][3], finite, already in the output frame -> the m picks DESIGN.md section 1.4 defines: pick 0 = start;
+ * every point carries D_i = the least fp32 d^2 = (dx dx + dy dy) + dz dz (no fused multiply-add) to the picks so far;
+ * pick t + 1 is the unpicked point of largest D_i, lowest index on ties (duplicates are taken in index order, no index
+ * twice).  Device outputs: out_idx int64 [m] in pick order, out_r2 fp32 [m] with out_r2[t] = max_i D_i after pick t
+ * (picked points count 0): the squared covering radius of the first t + 1 picks.
+ * 1 <= m <= n <= 2^24, 0 <= start < n.  ws: ma_farthest_point_sample_workspace_bytes(n, m) bytes (no device needed; 0
+ * for shapes out of range).  One kernel, cooperative above 8192 points; no allocation, no synchronisation.  Every
+ * choice is a maximum over unique integer keys: two calls give identical bits. */
+size_t ma_farthest_point_sample_workspace_bytes(int n, int m);
+int ma_farthest_point_sample(const float* xyz, int n, int m, int start, int64_t* out_idx, float* out_r2, void* ws,
+                             void* stream);
+/* Test and measurement hooks (tests/test_gpu_subsample.py, tools/bench_subsample.py): force the kernel path of every
+ * following call -- 0 chosen from n (default), 1 one CTA with the cloud in shared memory, 2 a cooperative grid with
+ * each CTA's slice in shared memory, 3 a cooperative grid with the slices in global memory; returns the previous
+ * setting (an unknown value changes nothing).  A forced path the device cannot hold makes the call fail.  The path
+ * the last successful call took (0 before any). */
+int ma_farthest_point_sample_set_path(int path);
+int ma_farthest_point_sample_last_path(void);
+
 /* number of kernels launched by the library since load (bench.py's gpu_launches) */
 unsigned long long ma_launch_count(void);
 

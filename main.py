@@ -3,6 +3,7 @@
     python main.py --input_type pc_normal --input_path pc_examples/mouse.npy --out_dir out [--sampling]
     python main.py --input_type pc --input_path scan.npy       # bare (N, 3) cloud: normals estimated on the GPU
     python main.py --input_type pc --input_path scan.npy --remove_outliers   # drop stray points / floaters first
+    python main.py --input_type pc --input_path scan.npy --subsample fps     # even coverage of uneven scan density
     torchrun --nproc-per-node 8 main.py --input_type pc_normal --input_dir pcs --batchsize_per_gpu 64
 
 Differences forced by the environment: no accelerate / hf_hub (there is no network) -- one process per
@@ -36,21 +37,36 @@ def _remove_outliers(xyz, path, outliers, n_points=4096):
     return idx.cpu().numpy()
 
 
-def _subsample_points(path, n_points=4096, outliers=None):
+def _farthest_points(xyz, path, n_points=4096):
+    """`--subsample fps`: the picks of farthest-point sampling (DESIGN.md section 1.4, on the GPU,
+    meshanything_b200.subsample) from a start drawn from the global numpy RNG, so --seed still selects the subset; one
+    line per input with the covering radius."""
+    from meshanything_b200.subsample import farthest_point_sample
+    n = xyz.shape[0]
+    idx, r2 = farthest_point_sample(xyz, n_points, np.random.randint(n))
+    print(f"{_uid_of(path)}: {n_points} of {n} points by farthest-point sampling; every point within "
+          f"{float(np.sqrt(r2[-1].item())):.4g} of one (output frame)")
+    return idx.cpu().numpy()
+
+
+def _subsample_points(path, n_points=4096, outliers=None, subsample='random'):
     """`--input_type pc_normal`: an .npy of >= 4096 (xyz, normal) rows; a random 4096-subset without replacement
-    (global numpy RNG, seeded by --seed as the reference does through accelerate.set_seed).  With `outliers` (the
-    keyword arguments of meshanything_b200.outliers.remove_outliers) the rows are first cleaned by their xyz."""
+    (global numpy RNG, seeded by --seed as the reference does through accelerate.set_seed), or with
+    subsample='fps' the farthest-point subset of the xyz columns.  With `outliers` (the keyword arguments of
+    meshanything_b200.outliers.remove_outliers) the rows are first cleaned by their xyz."""
     cloud = np.load(path)
     if outliers is not None:
         cloud = cloud[_remove_outliers(cloud[:, :3], path, outliers, n_points)]
     assert cloud.shape[0] >= n_points, "input pc_normal should have at least 4096 points"
+    if subsample == 'fps':
+        return cloud[_farthest_points(cloud[:, :3], path, n_points)]
     keep = np.random.choice(cloud.shape[0], n_points, replace=False)
     return cloud[keep]
 
 
-def _points_with_normals(path, n_points=4096, k=16, outliers=None):
+def _points_with_normals(path, n_points=4096, k=16, outliers=None, subsample='random'):
     """`--input_type pc`: a bare cloud (.npy (N, 3) or vertex-only .ply) of >= 4096 points.  Normals are estimated on
-    the GPU from all N points (meshanything_b200.normals), then the same random 4096-subset as `pc_normal` is drawn: the
+    the GPU from all N points (meshanything_b200.normals), then the same 4096-subset as `pc_normal` is drawn: the
     xyz-only copy of a file selects the points the file with normals selects under the same seed.  With `outliers`
     the cloud is cleaned first, and normals and subset come from the kept points."""
     from mesh_to_pc import load_points
@@ -62,7 +78,10 @@ def _points_with_normals(path, n_points=4096, k=16, outliers=None):
     if outliers is not None:
         xyz = xyz[_remove_outliers(xyz, path, outliers, n_points)]
     normals = estimate_normals(xyz, k).cpu().numpy()
-    keep = np.random.choice(xyz.shape[0], n_points, replace=False)
+    if subsample == 'fps':
+        keep = _farthest_points(xyz, path, n_points)
+    else:
+        keep = np.random.choice(xyz.shape[0], n_points, replace=False)
     return np.concatenate([xyz[keep], normals[keep].astype(xyz.dtype)], axis=1)
 
 
@@ -72,21 +91,33 @@ def _uid_of(path):
 
 _NO_MESH_OUTLIERS = ("--remove_outliers applies to point-cloud input (--input_type pc or pc_normal): the points of a "
                      "mesh are sampled from its surface and have no outliers")
+_NO_MESH_FPS = ("--subsample fps applies to point-cloud input (--input_type pc or pc_normal): the points of a mesh are "
+                "already sampled uniformly by area")
+SUBSAMPLERS = ('random', 'fps')
+
+
+def _check_subsample(input_type, subsample):
+    if subsample not in SUBSAMPLERS:
+        raise ValueError(f"--subsample must be one of {', '.join(SUBSAMPLERS)}, got {subsample!r}")
+    if subsample == 'fps' and input_type not in ('pc', 'pc_normal'):
+        raise ValueError(_NO_MESH_FPS)
 
 
 class Dataset:
     """Same contract as the reference's Dataset (main.py:15-58): items are {'pc_normal': fp16 (4096, 6), 'uid': str},
     coordinates centred on the bounding box and scaled to max |x| = 0.9995, unit normals asserted.  `outliers` (point
     clouds only): None, or the keyword arguments of meshanything_b200.outliers.remove_outliers, to clean every cloud
-    before normals and subset."""
+    before normals and subset.  `subsample` (point clouds only): 'random' (the reference's np.random.choice) or 'fps'
+    (farthest-point sampling on the GPU, DESIGN.md section 1.4)."""
 
-    def __init__(self, input_type, input_list, mc=False, outliers=None):
+    def __init__(self, input_type, input_list, mc=False, outliers=None, subsample='random'):
         if outliers is not None and input_type not in ('pc', 'pc_normal'):
             raise ValueError(_NO_MESH_OUTLIERS)
+        _check_subsample(input_type, subsample)
         if input_type == 'pc_normal':
-            clouds = [_subsample_points(p, outliers=outliers) for p in input_list]
+            clouds = [_subsample_points(p, outliers=outliers, subsample=subsample) for p in input_list]
         elif input_type == 'pc':
-            clouds = [_points_with_normals(p, outliers=outliers) for p in input_list]
+            clouds = [_points_with_normals(p, outliers=outliers, subsample=subsample) for p in input_list]
         elif input_type == 'mesh':
             if mc:
                 print("First Marching Cubes and then sample point cloud, need several minutes...")
@@ -134,6 +165,10 @@ def get_args():
     parser.add_argument('--outlier_neighbors', default=16, type=int)
     parser.add_argument('--outlier_std_ratio', default=2.0, type=float)
     parser.add_argument('--outlier_min_component', default=0.01, type=float)
+    # not in the reference: how the 4096 points the model sees are picked from a point cloud -- 'random' (the
+    # reference's np.random.choice) or 'fps', farthest-point sampling on the GPU, which covers a scan evenly whatever
+    # its density (DESIGN.md section 1.4; meshanything_b200.subsample)
+    parser.add_argument('--subsample', default='random', choices=SUBSAMPLERS)
     return parser.parse_args()
 
 
@@ -161,6 +196,7 @@ def check_args(args):
         if not (np.isfinite(args.outlier_std_ratio) and np.isfinite(args.outlier_min_component)
                 and args.outlier_min_component >= 0):
             raise ValueError("--outlier_std_ratio must be finite and --outlier_min_component finite and >= 0")
+    _check_subsample(args.input_type, getattr(args, 'subsample', 'random'))   # namespaces built without the flag
 
 
 def load_model(args, device=None):
@@ -284,7 +320,7 @@ if __name__ == "__main__":
         raise ValueError("input_dir or input_path must be provided.")
     np.random.seed(args.seed)
     torch.manual_seed(args.seed)
-    dataset = Dataset(args.input_type, input_list, args.mc, outliers=outlier_options(args))
+    dataset = Dataset(args.input_type, input_list, args.mc, outliers=outlier_options(args), subsample=args.subsample)
 
     bs = args.batchsize_per_gpu
     batches = [list(range(i, min(i + bs, len(dataset)))) for i in range(0, len(dataset), bs)]

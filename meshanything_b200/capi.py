@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+import operator
 import os
 from typing import Optional
 
@@ -51,7 +52,10 @@ EXPORTS = [
     "ma_estimate_normals_workspace_bytes", "ma_estimate_normals", "ma_estimate_normals_set_events",
     "ma_estimate_normals_last_rounds",
     "ma_remove_outliers_workspace_bytes", "ma_remove_outliers", "ma_remove_outliers_set_events",
+    "ma_farthest_point_sample_workspace_bytes", "ma_farthest_point_sample", "ma_farthest_point_sample_set_path",
+    "ma_farthest_point_sample_last_path",
 ]
+FPS_AUTO, FPS_ONE_CTA, FPS_GRID_SHARED, FPS_GRID_GLOBAL = 0, 1, 2, 3   # ma_farthest_point_sample_set_path
 
 
 def lib_path() -> str:
@@ -140,6 +144,13 @@ def lib():
                                      _vp]
     L.ma_remove_outliers_set_events.argtypes = [_vp]
     L.ma_remove_outliers_set_events.restype = None
+    L.ma_farthest_point_sample_workspace_bytes.argtypes = [C.c_int, C.c_int]
+    L.ma_farthest_point_sample_workspace_bytes.restype = C.c_size_t
+    L.ma_farthest_point_sample.argtypes = [_vp, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp, _vp]
+    L.ma_farthest_point_sample_set_path.argtypes = [C.c_int]
+    L.ma_farthest_point_sample_set_path.restype = C.c_int
+    L.ma_farthest_point_sample_last_path.argtypes = []
+    L.ma_farthest_point_sample_last_path.restype = C.c_int
     L.ma_linear_tc_f16.argtypes = [_vp, _vp, _vp, C.c_int, _vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _vp]
     L.ma_set_tensor_cores.argtypes = [C.c_int]
     L.ma_tensor_core_linear_counts.argtypes = [C.POINTER(C.c_ulonglong), C.POINTER(C.c_ulonglong)]
@@ -337,6 +348,46 @@ def remove_outliers(points: torch.Tensor, k: int = 16, std_ratio: float = 2.0, m
     st = stats.cpu().numpy()
     out = (idx[:int(st[6])], keep.bool(), st)
     return (*out, mean, knn) if want_terms else out
+
+
+def farthest_point_sample(points: torch.Tensor, m: int, start: int = 0):
+    """Farthest-point subsampling of a cloud (ma_farthest_point_sample; subsample.farthest_point_sample adds the frame
+    map).
+
+    points fp32 [N, 3], contiguous, on a CUDA device, finite, already in the output frame; 1 <= m <= N <= 2^24,
+    0 <= start < N.  Returns (picks int64 [m] in pick order, r2 fp32 [m]: r2[t] the squared covering radius of the first
+    t + 1 picks), both on the device.  Every bad input raises ValueError before anything is launched."""
+    if not isinstance(points, torch.Tensor):
+        raise ValueError(f"farthest_point_sample: points must be a torch tensor, got {type(points).__name__}")
+    if points.dim() != 2 or points.shape[1] != 3:
+        raise ValueError(f"farthest_point_sample: points [N, 3], got {tuple(points.shape)}")
+    if points.dtype != torch.float32:
+        raise ValueError(f"farthest_point_sample: points must be float32, got {points.dtype}")
+    if not points.is_contiguous():
+        raise ValueError("farthest_point_sample: points must be contiguous")
+    if not points.is_cuda:
+        raise ValueError("farthest_point_sample: points must live on a CUDA device (no CPU fallback)")
+    if isinstance(m, bool) or isinstance(start, bool):
+        raise ValueError("farthest_point_sample: m and start must be integers")
+    try:
+        m, start = operator.index(m), operator.index(start)
+    except TypeError:
+        raise ValueError(f"farthest_point_sample: m and start must be integers, got {m!r}, {start!r}") from None
+    n = points.shape[0]
+    if not 1 <= m <= n <= 1 << 24:
+        raise ValueError(f"farthest_point_sample: 1 <= m <= N <= 2^24, got N = {n}, m = {m}")
+    if not 0 <= start < n:
+        raise ValueError(f"farthest_point_sample: 0 <= start < N, got start = {start}, N = {n}")
+    if not bool(torch.isfinite(points).all()):
+        raise ValueError("farthest_point_sample: non-finite coordinates")
+    dev = points.device
+    ws = torch.empty(lib().ma_farthest_point_sample_workspace_bytes(n, m), dtype=torch.uint8, device=dev)
+    idx = torch.empty((m,), dtype=torch.int64, device=dev)
+    r2 = torch.empty((m,), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        check(lib().ma_farthest_point_sample(ptr(points), n, m, start, ptr(idx), ptr(r2), ptr(ws), stream_ptr()),
+              "ma_farthest_point_sample")
+    return idx, r2
 
 
 def tensor_core_linear_counts():
