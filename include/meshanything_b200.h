@@ -30,10 +30,6 @@ extern "C" {
 #define MA_EPI_NONE 0
 #define MA_EPI_RELU 1 /* OPTDecoderLayer activation_fn (opt-350m: relu) */
 #define MA_EPI_GELU 2 /* nn.GELU() exact erf: transformer_blocks.py:239, BERT intermediate */
-/* OR-ed into `epilogue`: the segmented accumulation order of the decoder's split-K layers (DESIGN.md section 3):
- * 16 segment dots (64-wide: out_proj, K = 1024; 256-wide: fc2, K = 4096) added with a balanced tree. */
-#define MA_LIN_SEG64 0x10
-#define MA_LIN_SEG256 0x20
 
 int ma_abi_version(void);
 const char* ma_last_error(void);
@@ -43,7 +39,7 @@ const char* ma_last_error(void);
 /* y[m][n] = fp16( dot(W[n][:], x[m][:]) + bias[n] ) then epilogue.  Replaces nn.Linear under fp16
  * autocast (every q/k/v/out_proj/fc1/fc2/lm_head/input_layer call of shape_opt.py:243,155 and HF
  * OPTDecoderLayer).  W [N][K] fp16 row-major, bias [N] fp16 or NULL, x [M][ldx] fp16, y [M][ldy]
- * fp16.  K % 256 == 0. */
+ * fp16.  K % 256 == 0.  Any other epilogue than MA_EPI_NONE / RELU / GELU is an error. */
 int ma_linear_f16(const void* W, const void* bias, const void* x, int ldx, void* y, int ldy, int M, int N, int K,
                   int epilogue, void* stream);
 
@@ -160,22 +156,13 @@ int ma_decode_slots_poll(int B, int tmax, void* ws, int32_t* finished_host, int3
 #define MA_GEN_NO_FAST 2    /* batch-1: use the general batched kernels instead of the fused GEMV path */
 #define MA_GEN_NO_PDL 4     /* batch-1 fast path without programmatic dependent launch */
 #define MA_GEN_NO_EARLY_EXIT 8
-#define MA_GEN_NO_MEGA 16    /* batch-1 greedy: per-phase kernels (decode_fast.cu) instead of the persistent kernel */
+#define MA_GEN_NO_MEGA 16    /* accepted and ignored: there is no persistent batch-1 kernel to opt out of; the bit
+                                stays reserved so that existing callers keep their meaning */
 #define MA_GEN_TC 64         /* batches: decoder GEMMs on the tensor cores (wgmma) -- logits within a tolerance of the
                                 canonical kernels instead of bit-exact ids; implied by sampling */
-#define MA_GEN_TRACE 32      /* persistent kernel records globaltimer stamps of CTA 0 at every phase boundary */
 
-/* Debug read-back (synchronises the device): what = 0 -> int error word of the persistent kernel (non-zero: a
- * hand-off between SMs timed out; value = 1 + the CTA that gave up first), what = 1 -> its uint64 trace stamps,
- * what = 2 -> the per-CTA stamps.  A time-out also makes the kernel stop emitting tokens and set out_lens[0] = -1. */
-int ma_decoder_debug(void* ws, int B, int tmax, int what, void* host_out, int nbytes);
-/* Test hook of the persistent kernel: bound of every in-kernel wait in ns (0 = keep; default: seconds) and fault
- * injection (fault = c + 1: CTA c withholds its out_proj rows from the third token on, so the hand-off times out). */
-void ma_mega_set_debug(unsigned long long timeout_ns, int fault);
-/* 1 if the persistent kernel can run on the current device (then batch-1 greedy decoding uses it unless
- * MA_GEN_NO_MEGA is set), 0 if batch-1 greedy decoding always takes the per-phase kernels there.  The kernel needs
- * every CTA to own fc1 and lm_head rows (at most 64 of each), the last 16 CTAs to own no out_proj rows, and a CTA's
- * rows to fit its shared memory: 147 SMs do, the 132 of an H100 do not. */
+/* Always 0: the library has no persistent decode kernel (batch-1 decoding runs the per-phase kernels of
+ * decode_fast.cu).  Kept for callers that query it. */
 int ma_decode_persistent_supported(void);
 
 

@@ -11,7 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIB_DIR, "libmeshanything_b200.so")
-SOURCES = ["gemm_canon.cu", "attention.cu", "attention_stream.cu", "elementwise.cu", "decode_fast.cu", "decode_mega.cu", "api.cu", "glue.cu", "gemm_tc.cu", "gemm_ws.cu", "attention_tc.cu", "api_encoder.cu", "surface.cu", "watertight.cu", "mesh_score.cu", "normals.cu", "outliers.cu", "subsample.cu"]
+SOURCES = ["gemm_canon.cu", "attention.cu", "attention_stream.cu", "elementwise.cu", "decode_fast.cu", "api.cu", "glue.cu", "gemm_tc.cu", "gemm_ws.cu", "attention_tc.cu", "api_encoder.cu", "surface.cu", "watertight.cu", "mesh_score.cu", "normals.cu", "outliers.cu", "subsample.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 

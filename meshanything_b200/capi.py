@@ -17,8 +17,7 @@ from . import build as _build
 
 MA_MAX_LAYERS = 32
 EPI_NONE, EPI_RELU, EPI_GELU = 0, 1, 2
-LIN_SEG64, LIN_SEG256 = 0x10, 0x20   # OR-ed into the epilogue: segmented order of the decoder's out_proj / fc2
-GEN_NO_GRAPH, GEN_NO_FAST, GEN_NO_PDL, GEN_NO_EARLY_EXIT, GEN_NO_MEGA, GEN_TRACE, GEN_TC = 1, 2, 4, 8, 16, 32, 64
+GEN_NO_GRAPH, GEN_NO_FAST, GEN_NO_PDL, GEN_NO_EARLY_EXIT, GEN_NO_MEGA, GEN_TC = 1, 2, 4, 8, 16, 64
 
 _vp = C.c_void_p
 
@@ -41,11 +40,11 @@ _lib = None
 EXPORTS = [
     "ma_abi_version", "ma_last_error", "ma_launch_count", "ma_linear_f16", "ma_layernorm",
     "ma_attention_scratch_bytes", "ma_attention_f16", "ma_attention_decode_f16", "ma_kv_cache_bytes", "ma_decoder_workspace_bytes",
-    "ma_decode_generate", "ma_decoder_debug", "ma_encoder_workspace_bytes", "ma_encoder_forward",
+    "ma_decode_generate", "ma_encoder_workspace_bytes", "ma_encoder_forward",
     "ma_detokenize_workspace_bytes", "ma_detokenize", "ma_linear_tc_f16", "ma_set_tensor_cores", "ma_sample_tokens",
     "ma_attention_tc_f16", "ma_transpose_heads_f16",
     "ma_decode_slots_init", "ma_decode_slot_prefill", "ma_decode_slots_step", "ma_decode_slots_poll",
-    "ma_mega_set_debug", "ma_linear_ws_set_mode", "ma_decode_slots_seek", "ma_decode_slot_stream", "ma_linear_ws_scratch_bytes", "ma_linear_ws_f16",
+    "ma_linear_ws_set_mode", "ma_decode_slots_seek", "ma_decode_slot_stream", "ma_linear_ws_scratch_bytes", "ma_linear_ws_f16",
     "ma_sample_surface_workspace_bytes", "ma_sample_surface", "ma_tensor_core_linear_counts", "ma_decode_persistent_supported",
     "ma_udf_grid", "ma_marching_cubes_workspace_bytes", "ma_marching_cubes_count", "ma_marching_cubes_emit",
     "ma_mesh_score_workspace_bytes", "ma_mesh_score",
@@ -107,9 +106,6 @@ def lib():
     L.ma_decode_slots_step.argtypes = [C.POINTER(DecoderWeights), C.c_int, C.c_int, C.c_int, C.c_int, C.c_int,
                                        C.POINTER(Sampling), C.c_int, C.c_int, _vp, _vp, _vp, C.c_int, _vp]
     L.ma_decode_slots_poll.argtypes = [C.c_int, C.c_int, _vp, _vp, _vp, _vp]
-    L.ma_decoder_debug.argtypes = [_vp, C.c_int, C.c_int, C.c_int, _vp, C.c_int]
-    L.ma_mega_set_debug.argtypes = [C.c_ulonglong, C.c_int]
-    L.ma_mega_set_debug.restype = None
     L.ma_decode_persistent_supported.argtypes = []
     L.ma_decode_persistent_supported.restype = C.c_int
     L.ma_encoder_workspace_bytes.argtypes = [C.c_int]

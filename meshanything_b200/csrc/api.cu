@@ -51,7 +51,6 @@ struct DecWs {
   void* attn_scratch_pre;  // prefill passes (M = 257 x sequences): its own area, because the layout (counters, then
   size_t attn_scratch_pre_bytes;  // partials) depends on M and a slot prefill may follow decode steps
   void* fast;
-  void* mega;
   void* tc_scratch;   // gemm_ws.cu: fp32 K-slice partials + tickets
   size_t total;
 };
@@ -86,7 +85,6 @@ static DecWs carve(void* base, int B, int tmax, int vocab) {
   w.attn_scratch_pre_bytes = attention_scratch_bytes(PREFIX * std::min(B, PREFILL_SEQS), NHEAD, PREFIX);
   w.attn_scratch_pre = take(w.attn_scratch_pre_bytes);
   w.fast = take(fast_workspace_bytes());
-  w.mega = take(mega_workspace_bytes());
   w.tc_scratch = take(linear_ws_scratch_bytes());
   w.total = off;
   return w;
@@ -399,10 +397,7 @@ int ma_decode_generate(const ma_decoder_weights* w, const float* prefix, int B, 
   const bool tc = use_tc(B, sa.do_sample, flags);
   if (tc) cudaMemsetAsync(ws.tc_scratch, 0, linear_ws_scratch_bytes(), st);   // tickets start at zero
   const bool fast = (B == 1) && !(flags & MA_GEN_NO_FAST);
-  // the persistent kernel needs 144 co-resident CTAs and tmax <= 15360 keys; otherwise the per-phase kernels run
-  bool mega = fast && !sa.do_sample && !(flags & MA_GEN_NO_MEGA) && mega_fits(tmax) && mega_supported();
   if (fast) sa.nkeys_next = fast_nkeys_ptr(ws.fast);
-  if (mega && mega_prepare(w, ws.mega, st)) mega = false;   // (message kept in ma_last_error)
 
   // ---- prefill: 257 prefix rows per sequence, PREFILL_SEQS sequences per pass
   for (int b0 = 0; b0 < B; b0 += PREFILL_SEQS) {
@@ -425,15 +420,7 @@ int ma_decode_generate(const ma_decoder_weights* w, const float* prefix, int B, 
   const unsigned long long whash = use_graph ? weights_hash(w) : 0;  // the struct is read at capture time
   bool flag_pending = false;
   int rc = 0;
-  if (mega) {
-    // persistent kernel: up to MEGA_STEPS tokens per launch; it returns early once the row has finished
-    const int MEGA_STEPS = 512;
-    for (int i = 1; i < max_new && rc == 0; i += MEGA_STEPS) {
-      rc = mega_enqueue(w, ws.s, tmax, (__half*)kv, ws.mega, sa, std::min(MEGA_STEPS, max_new - i), i - 1,
-                        (flags & MA_GEN_TRACE) ? 1 : 0, st);
-    }
-  }
-  for (int i = 1; i < max_new && rc == 0 && !mega; i++) {
+  for (int i = 1; i < max_new && rc == 0; i++) {
     const int ctx = PREFIX + i;                          // keys visible to this step (all rows advance together)
     const int bucket = (ctx + 1023) / 1024;              // attention grid size class
     const int max_keys = std::min(tmax, bucket * 1024);
@@ -630,18 +617,6 @@ int ma_decode_slots_poll(int B, int tmax, void* ws_, int32_t* finished_host, int
 }
 
 
-void ma_mega_set_debug(unsigned long long timeout_ns, int fault) { mega_set_debug(timeout_ns, fault); }
-int ma_decode_persistent_supported(void) { return mega_supported(); }
-
-int ma_decoder_debug(void* ws_, int B, int tmax, int what, void* host_out, int nbytes) {
-  DecWs ws = carve(ws_, B, tmax, 8195 + 61);
-  cudaDeviceSynchronize();
-  if (what == 0 && !mega_supported()) {   // the persistent kernel never runs on this device: nothing can time out
-    memset(host_out, 0, (size_t)nbytes);
-    return 0;
-  }
-  const char* src = (const char*)ws.mega + (what == 0 ? mega_error_flag_offset() : what == 1 ? mega_trace_offset() : mega_trace_cta_offset());
-  return cudaMemcpy(host_out, src, (size_t)nbytes, cudaMemcpyDeviceToHost) == cudaSuccess ? 0 : 1;
-}
+int ma_decode_persistent_supported(void) { return 0; }
 
 }  // extern "C"

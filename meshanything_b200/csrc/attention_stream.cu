@@ -11,8 +11,10 @@
 //     (cp.async.bulk onto mbarriers); the K slot is handed back right after the score pass, the V slot after the P.V
 //     pass, so the next chunk's rows are in flight while this one is being computed -- HBM never idles between chunks
 //     and no CTA launch / drain sits between two loads;
-//   * 8 consumer warps; the score butterfly is the transposing one of decode_mega.cu (7 shuffles for 8 rows, one exp
-//     per row), the same additions in the same tree as the plain xor butterfly;
+//   * 8 consumer warps; the score butterfly is lane-transposed: the 8 lanes of a row group hold partial dots of the
+//     group's 8 rows, and an xor-4,2,1 exchange that halves the rows each level leaves lane li with the finished score
+//     of row li (7 shuffles for 8 rows, one exp per row) -- the same additions in the same tree as the plain xor
+//     butterfly;
 //   * the k / v rows of the CURRENT token are taken straight from the qkv buffer by the lanes that own that key row and
 //     written to the cache from there (kv_append_kernel folded in: one launch less per layer);
 //   * chunk partials go to scratch with plain stores; a SEGMENT pays one fence + one atomic ticket (attention_kernel:

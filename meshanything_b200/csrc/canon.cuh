@@ -103,63 +103,6 @@ __device__ __forceinline__ float transpose_reduce32(float* v, int lane) {
   return v[0];
 }
 
-// The same with a chosen lane-bit order.  ORD = 1: xor-4,2,1,8,16 -- the segmented (64-wide) order of the decoder's
-// out_proj: the 8 lanes of a 64-element segment are reduced first, then the 4 segments of the 256-wide group as a
-// balanced tree.  On return lane l holds accumulator transpose_owner<ORD>(l) in v[0].
-template <int ORD>
-__device__ __forceinline__ float transpose_reduce32o(float* v, int lane) {
-#pragma unroll
-  for (int k = 0; k < 5; k++) {
-    const int s = 16 >> k;
-    const int m = ORD ? (k == 0 ? 4 : k == 1 ? 2 : k == 2 ? 1 : k == 3 ? 8 : 16) : s;
-    const bool up = (lane & m) != 0;
-#pragma unroll
-    for (int i = 0; i < s; i++) {
-      float mine = up ? v[i + s] : v[i];
-      float other = up ? v[i] : v[i + s];
-      float recv = __shfl_xor_sync(0xffffffffu, other, m);
-      v[i] = fadd(mine, recv);
-    }
-  }
-  return v[0];
-}
-template <int ORD>
-__device__ __forceinline__ int transpose_owner(int lane) {
-  if (!ORD) return lane;
-  return ((lane & 4) ? 16 : 0) | ((lane & 2) ? 8 : 0) | ((lane & 1) ? 4 : 0) | ((lane & 8) ? 2 : 0) | ((lane & 16) ? 1 : 0);
-}
-// every lane ends with the xor-4,2,1,8,16 sum (the seg-64 order) of the 32 lane partials
-__device__ __forceinline__ float warp_sum_seg64(float v) {
-  v = fadd(v, __shfl_xor_sync(0xffffffffu, v, 4));
-  v = fadd(v, __shfl_xor_sync(0xffffffffu, v, 2));
-  v = fadd(v, __shfl_xor_sync(0xffffffffu, v, 1));
-  v = fadd(v, __shfl_xor_sync(0xffffffffu, v, 8));
-  v = fadd(v, __shfl_xor_sync(0xffffffffu, v, 16));
-  return v;
-}
-// balanced binary tree over 16 values in index order, fed one value at a time (g = 0..15); lv = 4 level registers
-__device__ __forceinline__ float tree16_push(float v, int g, float* lv) {
-  if (g & 1) {
-    v = fadd(lv[0], v);
-    if (g & 2) {
-      v = fadd(lv[1], v);
-      if (g & 4) {
-        v = fadd(lv[2], v);
-        if (g & 8) v = fadd(lv[3], v); else lv[3] = v;
-      } else lv[2] = v;
-    } else lv[1] = v;
-  } else lv[0] = v;
-  return v;   // the total after g = 15
-}
-// the same over 4 values (g = 0..3): (v0 + v1) + (v2 + v3); lv = 2 registers
-__device__ __forceinline__ float tree4_push(float v, int g, float* lv) {
-  if (g == 0) lv[0] = v;
-  else if (g == 1) lv[0] = fadd(lv[0], v);
-  else if (g == 2) lv[1] = v;
-  else v = fadd(lv[0], fadd(lv[1], v));
-  return v;   // the total after g = 3
-}
-
 // pairwise left-to-right tree over n (<= 8) warp sums held in shared memory
 __device__ __forceinline__ float warp_tree(const float* s, int n) {
   float b[8];

@@ -103,17 +103,4 @@ size_t fast_workspace_bytes();
 int fast_step_enqueue(const ma_decoder_weights* w, SeqState s, int tmax, int max_keys, __half* kv, void* fast_ws,
                       const SampleArgs& sa, bool pdl, cudaStream_t st);
 
-
-// decode_mega.cu (batch-1 persistent kernel)
-size_t mega_workspace_bytes();
-int mega_prepare(const ma_decoder_weights* w, void* mega_ws, cudaStream_t st);
-int mega_enqueue(const ma_decoder_weights* w, SeqState s, int tmax, __half* kv, void* mega_ws, const SampleArgs& sa,
-                 int n_steps, int step_base, int trace, cudaStream_t st);
-int mega_supported();          // 1: the kernel's row split fits this device's SM count and shared memory
-bool mega_fits(int tmax);
-void mega_set_debug(unsigned long long timeout_ns, int fault);
-int mega_error_flag_offset();
-int mega_trace_offset();
-int mega_trace_cta_offset();
-
 }  // namespace ma

@@ -124,35 +124,4 @@ class Generator:
                                            flags, capi.stream_ptr())
         capi.check(rc, "ma_decode_generate")
         ids, lens = ids.clone(), lens.clone()          # the caller owns what it gets; the buffers are reused
-        self._last_lens = lens
         return (ids, lens, logits) if want_logits else (ids, lens)
-
-    def check(self):
-        """Raises if the last generate() failed on the device: the persistent decode kernel reports a timed-out
-        hand-off between SMs by writing lens = -1 and emitting no further tokens (synchronises the stream)."""
-        lens = getattr(self, "_last_lens", None)
-        if lens is not None and bool((lens < 0).any().item()):
-            code = self.mega_error()
-            raise RuntimeError(f"ma_decode_generate: the persistent decode kernel timed out waiting for another SM "
-                               f"(first CTA to give up: {code - 1}); no valid token sequence was produced")
-
-    def mega_error(self) -> int:
-        """non-zero if a hand-off of the persistent decode kernel timed out (synchronises the device): 1 + the CTA that
-        gave up first."""
-        out = C.c_int(0)
-        capi.check(capi.lib().ma_decoder_debug(capi.ptr(self.ws), self.batch, self.tmax, 0, C.byref(out), 4),
-                   "ma_decoder_debug")
-        return out.value
-
-    def mega_trace(self, n: int = 160):
-        """globaltimer stamps (ns) of CTA 0 at the phase boundaries of the last traced launch."""
-        buf = (C.c_uint64 * n)()
-        capi.check(capi.lib().ma_decoder_debug(capi.ptr(self.ws), self.batch, self.tmax, 1, buf, 8 * n),
-                   "ma_decoder_debug")
-        return list(buf)
-
-    def mega_trace_cta(self, n_cta: int = 147, n_stamps: int = 8):
-        buf = (C.c_uint64 * (n_cta * n_stamps))()
-        capi.check(capi.lib().ma_decoder_debug(capi.ptr(self.ws), self.batch, self.tmax, 2, buf, 8 * n_cta * n_stamps),
-                   "ma_decoder_debug")
-        return [[buf[c * n_stamps + k] for k in range(n_stamps)] for c in range(n_cta)]

@@ -45,7 +45,6 @@ def lib():
         build()
         L = C.CDLL(_LIB_PATH)
         L.orc_linear.argtypes = [u16p, u16p, u16p, C.c_int, C.c_int, C.c_int, C.c_int, u16p]
-        L.orc_linear_seg.argtypes = [u16p, u16p, u16p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, u16p]
         L.orc_layernorm.argtypes = [f32p, u16p, f32p, f32p, C.c_float, C.c_int, C.c_int, f32p, u16p]
         L.orc_attention.argtypes = [u16p, u16p, u16p, i32p, C.c_int, C.c_int, C.c_long, u16p]
         L.orc_exp.argtypes = [C.c_float]
@@ -90,18 +89,14 @@ def _p32(a: Optional[np.ndarray]):
 
 # ---------------------------------------------------------------- unit-level canonical ops
 
-def linear(w: torch.Tensor, b: Optional[torch.Tensor], x: torch.Tensor, relu: bool = False, seg: int = 0) -> torch.Tensor:
-    """fp16(x @ w.T + b) in the canonical order. w [N,K], x [M,K] -> fp16 [M,N].
-
-    seg = 64 (K = 1024) / 256 (K = 4096): the segmented order of the decoder's out_proj / fc2 (16 segment dots,
-    balanced tree)."""
-    assert seg in (0, 64, 256) and (seg == 0 or w.shape[1] == 16 * seg)
+def linear(w: torch.Tensor, b: Optional[torch.Tensor], x: torch.Tensor, relu: bool = False) -> torch.Tensor:
+    """fp16(x @ w.T + b) in the canonical order. w [N,K], x [M,K] -> fp16 [M,N]."""
     W, X = _h(w), _h(x)
     B = _h(b) if b is not None else None
     M, K = X.shape
     N = W.shape[0]
     y = np.empty((M, N), dtype=np.uint16)
-    lib().orc_linear_seg(_p16(W), _p16(B), _p16(X), M, N, K, int(relu), int(seg), _p16(y))
+    lib().orc_linear(_p16(W), _p16(B), _p16(X), M, N, K, int(relu), _p16(y))
     return torch.from_numpy(y.view(np.float16).copy())
 
 

@@ -119,74 +119,6 @@ static inline float dot_canon_T(const h16 *wT, const float *xT, int K) {
   return butterfly32(a);
 }
 
-/* one 256-wide group: lane l accumulates its 8 elements (j = 0..7) with fmaf from 0 */
-static inline void lane_chain8(const h16 *wT, const float *xT, float *a) {
-#ifdef ORC_SIMD
-  __m256 a0 = _mm256_setzero_ps(), a1 = a0, a2 = a0, a3 = a0;
-  for (int q = 0; q < 8; q++) {
-    const h16 *w = wT + q * 32;
-    const float *x = xT + q * 32;
-    a0 = _mm256_fmadd_ps(_mm256_cvtph_ps(_mm_loadu_si128((const __m128i *)(w))), _mm256_loadu_ps(x), a0);
-    a1 = _mm256_fmadd_ps(_mm256_cvtph_ps(_mm_loadu_si128((const __m128i *)(w + 8))), _mm256_loadu_ps(x + 8), a1);
-    a2 = _mm256_fmadd_ps(_mm256_cvtph_ps(_mm_loadu_si128((const __m128i *)(w + 16))), _mm256_loadu_ps(x + 16), a2);
-    a3 = _mm256_fmadd_ps(_mm256_cvtph_ps(_mm_loadu_si128((const __m128i *)(w + 24))), _mm256_loadu_ps(x + 24), a3);
-  }
-  _mm256_storeu_ps(a, a0);
-  _mm256_storeu_ps(a + 8, a1);
-  _mm256_storeu_ps(a + 16, a2);
-  _mm256_storeu_ps(a + 24, a3);
-#else
-  for (int l = 0; l < 32; l++) a[l] = 0.0f;
-  for (int q = 0; q < 8; q++)
-    for (int l = 0; l < 32; l++) a[l] = fmaf((float)wT[q * 32 + l], xT[q * 32 + l], a[l]);
-#endif
-}
-
-/* the four 64-wide segment dots of one 256-wide group: 8 lanes per segment, xor-4,2,1 butterfly */
-static inline void seg64_dots(const float *a, float *p) {
-  for (int q = 0; q < 4; q++) {
-    const float *b = a + 8 * q;
-    float c0 = b[0] + b[4], c1 = b[1] + b[5], c2 = b[2] + b[6], c3 = b[3] + b[7];
-    float d0 = c0 + c2, d1 = c1 + c3;
-    p[q] = d0 + d1;
-  }
-}
-
-/* balanced binary tree over 16 values in index order */
-static inline float tree16(const float *v) {
-  float a[8], b[4];
-  for (int i = 0; i < 8; i++) a[i] = v[2 * i] + v[2 * i + 1];
-  for (int i = 0; i < 4; i++) b[i] = a[2 * i] + a[2 * i + 1];
-  return (b[0] + b[1]) + (b[2] + b[3]);
-}
-
-/* Segmented dot -- the order a split-K partition of out_proj / fc2 across SM groups produces.  Round 2 built and
- * measured that partition (DESIGN.md section 4.1.2: slower than the row split, so the decoder does NOT use it); the
- * order stays available through orc_linear_seg / MA_LIN_SEG64 / MA_LIN_SEG256 and is unit-tested.  K is cut into 16
- * segments (seg = 64: K = 1024, out_proj -- one segment per attention head; seg = 256: K = 4096, fc2 -- one segment
- * per 256 fc1 rows).  Each segment dot is reduced on its own (lanes run their 8-element fmaf chain from 0; seg 64:
- * xor-4,2,1 butterfly over the segment's 8 lanes; seg 256: the 32-lane butterfly); the 16 segment dots are added
- * with a balanced binary tree in index order. */
-static inline float dot_seg_T(const h16 *wT, const float *xT, int K, int seg) {
-  float v[16], a[32];
-  if (seg == 64) { /* K == 1024 */
-    for (int g = 0; g < 4; g++) {
-      lane_chain8(wT + 256 * g, xT + 256 * g, a);
-      seg64_dots(a, v + 4 * g);
-    }
-  } else { /* seg == 256, K == 4096 */
-    for (int g = 0; g < 16; g++) {
-      lane_chain8(wT + 256 * g, xT + 256 * g, a);
-      v[g] = butterfly32(a);
-    }
-  }
-  (void)K;
-  return tree16(v);
-}
-static inline float dot_any_T(const h16 *wT, const float *xT, int K, int seg) {
-  return seg ? dot_seg_T(wT, xT, K, seg) : dot_canon_T(wT, xT, K);
-}
-
 /* pairwise left-to-right tree over n warp sums (n = 8: ((0+1)+(2+3))+((4+5)+(6+7)); n = 6: ((0+1)+(2+3))+(4+5)) */
 static float warp_tree(const float *s, int n) {
   float buf[16];
@@ -293,8 +225,8 @@ static void attention_head_canon(const h16 *q, const h16 *Kc, const h16 *Vc, lon
 /* ------------------------------------------------------------------ unit-level entry points */
 
 /* y[M][N] = fp16(dot(W[n], x[m]) + b[n]) (+relu); W [N][K], x [M][K], b [N] or NULL, all fp16 */
-void orc_linear_seg(const uint16_t *W_, const uint16_t *b_, const uint16_t *x_, int M, int N, int K, int relu,
-                    int seg, uint16_t *y_) {
+void orc_linear(const uint16_t *W_, const uint16_t *b_, const uint16_t *x_, int M, int N, int K, int relu,
+                uint16_t *y_) {
   const h16 *W = (const h16 *)W_, *b = (const h16 *)b_, *x = (const h16 *)x_;
   h16 *y = (h16 *)y_;
   float *xT = (float *)malloc(sizeof(float) * (size_t)M * K);
@@ -307,7 +239,7 @@ void orc_linear_seg(const uint16_t *W_, const uint16_t *b_, const uint16_t *x_, 
       transpose_row_h16(W + (size_t)n * K, wT, K);
       float bf = b ? (float)b[n] : 0.0f;
       for (int m = 0; m < M; m++) {
-        float acc = dot_any_T(wT, xT + (size_t)m * K, K, seg);
+        float acc = dot_canon_T(wT, xT + (size_t)m * K, K);
         h16 r = (h16)(acc + bf);
         if (relu && (float)r < 0.0f) r = (h16)0.0f;
         y[(size_t)m * N + n] = r;
@@ -316,10 +248,6 @@ void orc_linear_seg(const uint16_t *W_, const uint16_t *b_, const uint16_t *x_, 
     free(wT);
   }
   free(xT);
-}
-void orc_linear(const uint16_t *W_, const uint16_t *b_, const uint16_t *x_, int M, int N, int K, int relu,
-                uint16_t *y_) {
-  orc_linear_seg(W_, b_, x_, M, N, K, relu, 0, y_);
 }
 
 /* rows of width W: h = x (+ float(res16)); y = LN(h); outputs fp32 y and fp16 y */
@@ -471,12 +399,12 @@ void orc_dec_destroy(void *h) {
 }
 
 /* y16[m][n] = fp16(dot + b) for M rows with weight reuse; xT [M][K] lane-transposed fp32 */
-static void linear_T(const h16 *wT, const h16 *b, const float *xT, int M, int N, int K, int relu, int seg, h16 *y) {
+static void linear_T(const h16 *wT, const h16 *b, const float *xT, int M, int N, int K, int relu, h16 *y) {
 #pragma omp parallel for schedule(static)
   for (int n = 0; n < N; n++) {
     float bf = b ? (float)b[n] : 0.0f;
     for (int m = 0; m < M; m++) {
-      float acc = dot_any_T(wT + (size_t)n * K, xT + (size_t)m * K, K, seg);
+      float acc = dot_canon_T(wT + (size_t)n * K, xT + (size_t)m * K, K);
       h16 r = (h16)(acc + bf);
       if (relu && (float)r < 0.0f) r = (h16)0.0f;
       y[(size_t)m * N + n] = r;
@@ -514,9 +442,9 @@ static void run_tokens(orc_dec *o, float *hid, int M, uint16_t *logits_, int log
     orc_layer *l = &o->L[li];
     h16 *kc = o->kc + (size_t)li * NHEAD * T * HD, *vc = o->vc + (size_t)li * NHEAD * T * HD;
     to_xT(hid, xT, M, HID);
-    linear_T(l->wq, l->bq, xT, M, HID, HID, 0, 0, q);
-    linear_T(l->wk, l->bk, xT, M, HID, HID, 0, 0, k);
-    linear_T(l->wv, l->bv, xT, M, HID, HID, 0, 0, v);
+    linear_T(l->wq, l->bq, xT, M, HID, HID, 0, q);
+    linear_T(l->wk, l->bk, xT, M, HID, HID, 0, k);
+    linear_T(l->wv, l->bv, xT, M, HID, HID, 0, v);
     for (int m = 0; m < M; m++)
       for (int hh = 0; hh < NHEAD; hh++) {
         memcpy(kc + ((size_t)hh * T + t0 + m) * HD, k + (size_t)m * HID + hh * HD, HD * sizeof(h16));
@@ -528,7 +456,7 @@ static void run_tokens(orc_dec *o, float *hid, int M, uint16_t *logits_, int log
         attention_head_canon(q + (size_t)m * HID + hh * HD, kc + (size_t)hh * T * HD, vc + (size_t)hh * T * HD, HD,
                              t0 + m + 1, a + (size_t)m * HID + hh * HD);
     h16_to_xT(a, xT, M, HID);
-    linear_T(l->wo, l->bo, xT, M, HID, HID, 0, 0, y);
+    linear_T(l->wo, l->bo, xT, M, HID, HID, 0, y);
 #pragma omp parallel for schedule(static)
     for (int m = 0; m < M; m++) {
       float h[HID];
@@ -536,9 +464,9 @@ static void run_tokens(orc_dec *o, float *hid, int M, uint16_t *logits_, int log
       layernorm_canon(h, l->ln1g, l->ln1b, MA_LN_EPS, hid + (size_t)m * HID, HID);
     }
     to_xT(hid, xT, M, HID);
-    linear_T(l->w1, l->b1, xT, M, FFN, HID, 1, 0, f);
+    linear_T(l->w1, l->b1, xT, M, FFN, HID, 1, f);
     h16_to_xT(f, xT, M, FFN);
-    linear_T(l->w2, l->b2, xT, M, HID, FFN, 0, 0, y);
+    linear_T(l->w2, l->b2, xT, M, HID, FFN, 0, y);
 #pragma omp parallel for schedule(static)
     for (int m = 0; m < M; m++) {
       float h[HID];
@@ -550,10 +478,10 @@ static void run_tokens(orc_dec *o, float *hid, int M, uint16_t *logits_, int log
   if (logits) {
     if (logits_all) {
       to_xT(hid, xT, M, HID);
-      linear_T(o->lm_head, NULL, xT, M, o->vocab, HID, 0, 0, logits);
+      linear_T(o->lm_head, NULL, xT, M, o->vocab, HID, 0, logits);
     } else {
       to_xT(hid + (size_t)(M - 1) * HID, xT, 1, HID);
-      linear_T(o->lm_head, NULL, xT, 1, o->vocab, HID, 0, 0, logits);
+      linear_T(o->lm_head, NULL, xT, 1, o->vocab, HID, 0, logits);
     }
   }
   o->t = t0 + M;

@@ -2,7 +2,7 @@
 import pytest
 import torch
 
-from tests.util import decoder_sd, random_prefix, skip_unless_persistent
+from tests.util import decoder_sd, random_prefix
 
 gpu = pytest.mark.gpu
 NL = 3          # layers of the small synthetic decoder used by most cases
@@ -30,59 +30,22 @@ def test_tok_table_matches_oracle(small):
 
 
 @gpu
-@pytest.mark.parametrize("flags", [0, 16, 16 | 4, 16 | 1, 2, 2 | 1])
+@pytest.mark.parametrize("flags", [0, 16, 4, 1, 2, 2 | 1])
 def test_greedy_bit_exact_vs_oracle(small, flags):
     """free-running greedy decode: token ids and every step's fp16 logits equal the oracle's.
-    flags: 0 persistent kernel, 16 per-phase kernels + PDL, 16|4 without PDL, |1 without CUDA graph, 2 batched kernels."""
+    flags: 0 per-phase kernels + PDL, 16 the same (MA_GEN_NO_MEGA is accepted and ignored), 4 without PDL, |1 without
+    CUDA graph, 2 batched kernels."""
     from meshanything_b200.decoder import Generator
-    skip_unless_persistent(flags)
     _, arena, oracle = small
     prefix = random_prefix(1, seed=3)
     gen = Generator(arena, 1, 257 + NEW)
     ids, lens, logits = gen.generate(prefix.to(_dev()), NEW, want_logits=True, flags=flags)
     torch.cuda.synchronize()
-    if flags == 0:
-        assert gen.mega_error() == 0
     ref_ids, ref_logits = oracle.generate(prefix[0], NEW, keep_logits=True)
     assert ids[0].cpu().tolist() == ref_ids
     for i, rl in enumerate(ref_logits):
         assert torch.equal(logits[i, 0].cpu().view(torch.int16), rl.view(torch.int16)), f"logits differ at step {i}"
     assert int(lens[0]) == NEW
-
-
-@gpu
-def test_persistent_kernel_timeout_is_an_error(small):
-    """Fault injection (ma_mega_set_debug): CTA 37 withholds its out_proj rows from the third token on.  The
-    readers' wait must time out, the kernel must stop emitting tokens, report lens = -1 and an error word, and
-    Generator.check() (called by MeshAnything.forward) must raise -- never a silently wrong sequence.  Afterwards the
-    same generator works again."""
-    import time
-    from meshanything_b200 import capi
-    from meshanything_b200.decoder import Generator
-    skip_unless_persistent(0)
-    _, arena, oracle = small
-    prefix = random_prefix(1, seed=3)
-    gen = Generator(arena, 1, 257 + NEW)
-    good, _ = gen.generate(prefix.to(_dev()), NEW)
-    gen.check()
-    good = good[0].cpu().tolist()
-    capi.lib().ma_mega_set_debug(20_000_000, 37 + 1)      # 20 ms per wait
-    try:
-        t0 = time.time()
-        ids, lens = gen.generate(prefix.to(_dev()), NEW, pad_id=2)
-        torch.cuda.synchronize()
-        assert time.time() - t0 < 5.0, "a time-out must not take seconds"
-        assert int(lens[0]) == -1
-        assert gen.mega_error() != 0                        # 1 + the CTA that gave up first
-        got = ids[0].cpu().tolist()
-        assert got[:3] == good[:3] and all(t == 2 for t in got[3:]), got[:8]   # nothing emitted after the failure
-        with pytest.raises(RuntimeError, match="timed out"):
-            gen.check()
-    finally:
-        capi.lib().ma_mega_set_debug(2_000_000_000, 0)
-    again, lens = gen.generate(prefix.to(_dev()), NEW)
-    gen.check()
-    assert again[0].cpu().tolist() == good and int(lens[0]) == NEW
 
 
 @gpu
@@ -148,7 +111,10 @@ def test_eos_and_padding(small):
     assert int(lens1[0]) == len(ref_ids)
 
 
-def _teacher_forced_logits(small, flags):
+@gpu
+def test_teacher_forced_logits(small):
+    """forced ids (incl. specials 0/1/2, which take the extra_embeds path) give the oracle's logits, on the per-phase
+    kernels (flags 0) and the batched kernels (flags 2)."""
     from meshanything_b200.decoder import Generator
     _, arena, oracle = small
     prefix = random_prefix(1, seed=8)
@@ -156,26 +122,12 @@ def _teacher_forced_logits(small, flags):
     n = len(forced)
     gen = Generator(arena, 1, 257 + n)
     f = torch.tensor([forced], dtype=torch.int32)
-    ids, lens, logits = gen.generate(prefix.to(_dev()), n, forced_ids=f, want_logits=True, eos_id=-1, flags=flags)
     _, ref_logits = oracle.generate(prefix[0], n, eos_id=-1, forced=forced, keep_logits=True)
-    assert ids[0].cpu().tolist() == forced
-    for i in range(n):
-        assert torch.equal(logits[i, 0].cpu().view(torch.int16), ref_logits[i].view(torch.int16)), (flags, i)
-
-
-@gpu
-def test_teacher_forced_logits(small):
-    """forced ids (incl. specials 0/1/2, which take the extra_embeds path) give the oracle's logits, on the per-phase
-    kernels (flags 16) and the batched kernels (flags 2)."""
-    for flags in (16, 2):
-        _teacher_forced_logits(small, flags)
-
-
-@gpu
-def test_teacher_forced_logits_persistent_kernel(small):
-    """the same on the persistent kernel (flags 0), where the device can host it."""
-    skip_unless_persistent(0)
-    _teacher_forced_logits(small, 0)
+    for flags in (0, 2):
+        ids, lens, logits = gen.generate(prefix.to(_dev()), n, forced_ids=f, want_logits=True, eos_id=-1, flags=flags)
+        assert ids[0].cpu().tolist() == forced
+        for i in range(n):
+            assert torch.equal(logits[i, 0].cpu().view(torch.int16), ref_logits[i].view(torch.int16)), (flags, i)
 
 
 @gpu
@@ -212,30 +164,17 @@ def test_tensor_core_decoder_logits_within_tolerance(small):
     print("tensor-core decoder: max |logit diff| vs oracle", worst)
 
 
-def _long_context_crosses_chunks(small, flags):
+@gpu
+def test_long_context_crosses_chunks(small):
+    """600 new tokens: the context crosses three 256-key attention chunks (257 -> 857); per-phase kernels."""
     from meshanything_b200.decoder import Generator
     _, arena, oracle = small
     prefix = random_prefix(1, seed=13)
     n = 600
     ref_ids, _ = oracle.generate(prefix[0], n)
     gen = Generator(arena, 1, 257 + n)
-    ids, _ = gen.generate(prefix.to(_dev()), n, flags=flags)
-    assert ids[0].cpu().tolist() == ref_ids, flags
-    if flags == 0:
-        assert gen.mega_error() == 0
-
-
-@gpu
-def test_long_context_crosses_chunks(small):
-    """600 new tokens: the context crosses three 256-key attention chunks (257 -> 857); per-phase kernels."""
-    _long_context_crosses_chunks(small, 16)
-
-
-@gpu
-def test_long_context_crosses_chunks_persistent_kernel(small):
-    """the same on the persistent kernel, where the device can host it."""
-    skip_unless_persistent(0)
-    _long_context_crosses_chunks(small, 0)
+    ids, _ = gen.generate(prefix.to(_dev()), n)
+    assert ids[0].cpu().tolist() == ref_ids
 
 
 @gpu
@@ -279,7 +218,12 @@ def test_full_depth_config1_golden():
         assert got == ref
 
 
-def _full_depth_config2_golden(flags):
+@gpu
+@pytest.mark.slow
+def test_full_depth_config2_golden():
+    """BASELINE.json configs[1] parity: 24 layers, 800-face cap (7202 new tokens, contexts up to 7458), batch 1, greedy.
+    The free-running token ids on the per-phase kernels equal the CPU oracle's (tests/golden/decoder_greedy_seed0_F800.json,
+    generated by tests/golden/make_golden.py greedy800)."""
     import json, os
     from meshanything_b200.decoder import DecoderArena, Generator
     gold = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "decoder_greedy_seed0_F800.json")))["ids"]
@@ -287,54 +231,11 @@ def _full_depth_config2_golden(flags):
     prefix = random_prefix(1, seed=1).to(_dev())
     n = 800 * 9 + 2
     gen = Generator(arena, 1, 257 + n)
-    ids, lens = gen.generate(prefix, n, flags=flags)
+    ids, lens = gen.generate(prefix, n)
     got = ids[0].cpu().tolist()
     first_bad = next((i for i, (a, b) in enumerate(zip(got, gold)) if a != b), None)
-    assert first_bad is None, f"flags={flags}: first divergence at step {first_bad}"
+    assert first_bad is None, f"first divergence at step {first_bad}"
     assert int(lens[0]) == n
-    if flags == 0:
-        assert gen.mega_error() == 0
-
-
-@gpu
-@pytest.mark.slow
-def test_full_depth_config2_golden():
-    """BASELINE.json configs[1] parity: 24 layers, 800-face cap (7202 new tokens, contexts up to 7458), batch 1, greedy.
-    The free-running token ids on the per-phase kernels equal the CPU oracle's (tests/golden/decoder_greedy_seed0_F800.json,
-    generated by tests/golden/make_golden.py greedy800)."""
-    _full_depth_config2_golden(16)
-
-
-@gpu
-@pytest.mark.slow
-def test_full_depth_config2_golden_persistent_kernel():
-    """the same on the persistent kernel, where the device can host it."""
-    skip_unless_persistent(0)
-    _full_depth_config2_golden(0)
-
-
-def _long_context_config5_golden(flags, batched):
-    import json, os
-    from meshanything_b200.decoder import DecoderArena, Generator
-    g = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "decoder_greedy_seed0_F1600.json")))
-    gold, NL, eos = g["ids"], g["n_layers"], g.get("eos_id", 1)
-    assert len(gold) == 1600 * 9 + 2
-    arena = DecoderArena(decoder_sd(NL), _dev())
-    prefix = random_prefix(1, seed=1).to(_dev())
-    n = 1600 * 9 + 2
-    gen = Generator(arena, 1, 257 + n)
-    ids, lens = gen.generate(prefix, n, flags=flags, eos_id=eos)
-    got = ids[0].cpu().tolist()
-    first_bad = next((i for i, (a, b) in enumerate(zip(got, gold)) if a != b), None)
-    assert first_bad is None, f"flags={flags}: first divergence at step {first_bad}"
-    assert int(lens[0]) == n
-    if flags == 0:
-        assert gen.mega_error() == 0
-    if batched:
-        two = torch.cat([prefix, random_prefix(1, seed=5).to(_dev())], dim=0)
-        gen2 = Generator(arena, 2, 257 + n)
-        ids2, _ = gen2.generate(two, n, eos_id=eos)
-        assert ids2[0].cpu().tolist() == gold
 
 
 @gpu
@@ -344,15 +245,24 @@ def test_long_context_config5_golden():
     attention chunks).  First 4 layers of the synthetic decoder; ids equal the CPU oracle's
     (tests/golden/decoder_greedy_seed0_F1600.json, make_golden.py greedy1600) for the per-phase kernels and for a batch
     of 2 on the batched kernels (row 0 = the golden prefix, row 1 another prefix: rows are independent)."""
-    _long_context_config5_golden(16, batched=True)
-
-
-@gpu
-@pytest.mark.slow
-def test_long_context_config5_golden_persistent_kernel():
-    """the same length on the persistent kernel (four rounds of attention items), where the device can host it."""
-    skip_unless_persistent(0)
-    _long_context_config5_golden(0, batched=False)
+    import json, os
+    from meshanything_b200.decoder import DecoderArena, Generator
+    g = json.load(open(os.path.join(os.path.dirname(__file__), "golden", "decoder_greedy_seed0_F1600.json")))
+    gold, NL, eos = g["ids"], g["n_layers"], g.get("eos_id", 1)
+    assert len(gold) == 1600 * 9 + 2
+    arena = DecoderArena(decoder_sd(NL), _dev())
+    prefix = random_prefix(1, seed=1).to(_dev())
+    n = 1600 * 9 + 2
+    gen = Generator(arena, 1, 257 + n)
+    ids, lens = gen.generate(prefix, n, eos_id=eos)
+    got = ids[0].cpu().tolist()
+    first_bad = next((i for i, (a, b) in enumerate(zip(got, gold)) if a != b), None)
+    assert first_bad is None, f"first divergence at step {first_bad}"
+    assert int(lens[0]) == n
+    two = torch.cat([prefix, random_prefix(1, seed=5).to(_dev())], dim=0)
+    gen2 = Generator(arena, 2, 257 + n)
+    ids2, _ = gen2.generate(two, n, eos_id=eos)
+    assert ids2[0].cpu().tolist() == gold
 
 
 @gpu
