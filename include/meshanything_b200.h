@@ -199,6 +199,38 @@ int ma_attention_tc_f16(const void* q, int ldq, const void* K, const void* Vt, l
 int ma_transpose_heads_f16(const void* src, int ld, int col0, int head_stride, int H, int n, long Tpad, int n_slots,
                            void* dst, void* stream);
 
+/* ---- test hooks: the glue kernels of ma_encoder_forward / ma_detokenize (csrc/glue.cu), one entry point each -------
+ * The library's own callers launch these kernels directly; the entry points exist so that tests can compare each one
+ * with a plain restatement.  Each returns non-zero, launching nothing, on a null pointer (optional ones noted), a
+ * non-positive count, or a width or alignment its vector accesses cannot take.
+ *   ma_fourier_embed_f16  pc fp16 [rows][6] (xyz | normal) -> out fp16 [rows][256] = [xyz | sin(x 2^j) coordinate-major,
+ *                         j = 0..7 (24) | cos (24) | normal | 0 ...] (a1); out 8-byte aligned.
+ *   ma_scatter_heads_f16  dst[((slot H + h) T + t) 64 + d] = src[m ld + col0 + h head_stride + d] for m < rows, h < H,
+ *                         d < 64, slot = m / rows_per_slot, t = m % rows_per_slot; ld, col0, head_stride multiples of 8,
+ *                         both pointers 16-byte aligned.
+ *   ma_residual_add       x32 fp32 [n] += float(y) (x16 NULL), or x16 fp16 [n] = fp16(float(x16) + float(y)) (x32 NULL);
+ *                         n % 4 == 0.
+ *   ma_convert_rows       dst[r ldd + c] = (dst type) src[(src_rows_mod ? r % src_rows_mod : r) lds + c] for r < rows,
+ *                         c < cols; fp16 (flag 1) or fp32 (flag 0) on either side, round to nearest even; cols % 4 == 0.
+ *   ma_add_table          out fp32 [rows][768] = (mask && !mask[r] ? 0 : float(y16[r])) + table[r % table_rows]; mask
+ *                         int32 [rows] optional.
+ *   ma_gather_codes       gen_ids int32 [B][max_new] -> ids_out int32 [B][F][9] (optional; id - 3, -1 for the specials
+ *                         0, 1, 2 and beyond position max_new - 2), mask int32 [B][F] (all 9 present), code16 fp16
+ *                         [B][F][3][1024] = fp16((c0 + c1) + c2) of the vertex's three codebook rows (absent = 0).
+ *   ma_coords             logits fp16 [faces][9][128] -> xyz fp32 [faces][9] = bin / 128 - 0.5, bin the lowest index of
+ *                         the largest logit (NaN logits are skipped); faces with mask 0 hold the quiet NaN 0x7fc00000. */
+int ma_fourier_embed_f16(const void* pc, long rows, void* out, void* stream);
+int ma_scatter_heads_f16(const void* src, int ld, int col0, int head_stride, int H, int rows_per_slot, long T, void* dst,
+                         long rows, void* stream);
+int ma_residual_add(float* x32, void* x16, const void* y, long n, void* stream);
+int ma_convert_rows(const void* src, int src_f16, long lds, void* dst, int dst_f16, long ldd, long rows, int cols,
+                    long src_rows_mod, void* stream);
+int ma_add_table(const void* y16, const int* mask, const float* table, int table_rows, float* out, long rows,
+                 void* stream);
+int ma_gather_codes(const int32_t* gen_ids, int max_new, int B, int F, const float* codebook, void* code16, int* mask,
+                    int32_t* ids_out, void* stream);
+int ma_coords(const void* logits, const int* mask, float* xyz, long faces, void* stream);
+
 /* ---- Michelangelo point-cloud encoder (a1-a8) ----------------------------------------------- */
 
 typedef struct { /* ResidualAttentionBlock, transformer_blocks.py:77-115 (qkv_bias: false) */

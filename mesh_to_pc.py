@@ -53,6 +53,8 @@ class SimpleMesh:
                 elif p[0] == "f":
                     ids = [int(x.split("/")[0]) for x in p[1:]]
                     ids = [i - 1 if i > 0 else len(vs) + i for i in ids]
+                    if any(not 0 <= i < len(vs) for i in ids):   # vertices are declared before the faces using them
+                        raise ValueError(f"{path}: face {line.strip()!r} refers to a vertex outside 1..{len(vs)}")
                     for k in range(1, len(ids) - 1):          # fan triangulation
                         fs.append([ids[0], ids[k], ids[k + 1]])
         return SimpleMesh(vs, fs)

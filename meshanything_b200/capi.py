@@ -53,6 +53,8 @@ EXPORTS = [
     "ma_remove_outliers_workspace_bytes", "ma_remove_outliers", "ma_remove_outliers_set_events",
     "ma_farthest_point_sample_workspace_bytes", "ma_farthest_point_sample", "ma_farthest_point_sample_set_path",
     "ma_farthest_point_sample_last_path",
+    "ma_fourier_embed_f16", "ma_scatter_heads_f16", "ma_residual_add", "ma_convert_rows", "ma_add_table",
+    "ma_gather_codes", "ma_coords",
 ]
 FPS_AUTO, FPS_ONE_CTA, FPS_GRID_SHARED, FPS_GRID_GLOBAL = 0, 1, 2, 3   # ma_farthest_point_sample_set_path
 
@@ -147,6 +149,13 @@ def lib():
     L.ma_farthest_point_sample_set_path.restype = C.c_int
     L.ma_farthest_point_sample_last_path.argtypes = []
     L.ma_farthest_point_sample_last_path.restype = C.c_int
+    L.ma_fourier_embed_f16.argtypes = [_vp, C.c_long, _vp, _vp]
+    L.ma_scatter_heads_f16.argtypes = [_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_long, _vp, C.c_long, _vp]
+    L.ma_residual_add.argtypes = [_vp, _vp, _vp, C.c_long, _vp]
+    L.ma_convert_rows.argtypes = [_vp, C.c_int, C.c_long, _vp, C.c_int, C.c_long, C.c_long, C.c_int, C.c_long, _vp]
+    L.ma_add_table.argtypes = [_vp, _vp, _vp, C.c_int, _vp, C.c_long, _vp]
+    L.ma_gather_codes.argtypes = [_vp, C.c_int, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp]
+    L.ma_coords.argtypes = [_vp, _vp, _vp, C.c_long, _vp]
     L.ma_linear_tc_f16.argtypes = [_vp, _vp, _vp, C.c_int, _vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, _vp]
     L.ma_set_tensor_cores.argtypes = [C.c_int]
     L.ma_tensor_core_linear_counts.argtypes = [C.POINTER(C.c_ulonglong), C.POINTER(C.c_ulonglong)]
@@ -195,9 +204,33 @@ def linear_f16(w: torch.Tensor, bias: Optional[torch.Tensor], x: torch.Tensor, e
 
 def sample_surface(vertices: torch.Tensor, faces: torch.Tensor, n_samples: int, seed: int = 0,
                    want_index: bool = False):
-    """Area-weighted surface samples + face normals on the GPU: fp16 [n_samples, 6] (and the face of every sample)."""
+    """Area-weighted surface samples + face normals on the GPU: fp16 [n_samples, 6] (and the face of every sample).
+
+    vertices [V, 3] finite, faces [F, 3] with indices in [0, V), F >= 1, n_samples >= 1, 0 <= seed < 2^64.  Every bad
+    input raises ValueError before anything is launched.  A mesh whose faces all have zero area gets the last face and a
+    zero normal for every sample (DESIGN.md section 1.5)."""
     _need_cuda(vertices, faces)
+    if vertices.dim() != 2 or vertices.shape[1] != 3 or faces.dim() != 2 or faces.shape[1] != 3:
+        raise ValueError(f"sample_surface: vertices [V, 3] and faces [F, 3], got {tuple(vertices.shape)} and "
+                         f"{tuple(faces.shape)}")
+    if faces.shape[0] < 1:
+        raise ValueError("sample_surface: a mesh without faces has no surface to sample")
+    try:
+        n_samples, seed = operator.index(n_samples), operator.index(seed)
+    except TypeError:
+        raise ValueError(f"sample_surface: n_samples and seed must be integers, got {n_samples!r}, {seed!r}") from None
+    if not 1 <= n_samples < 1 << 31:
+        raise ValueError(f"sample_surface: 1 <= n_samples < 2^31, got {n_samples}")
+    if not 0 <= seed < 1 << 64:
+        raise ValueError(f"sample_surface: 0 <= seed < 2^64, got {seed}")
+    if faces.dtype.is_floating_point or faces.dtype.is_complex or faces.dtype == torch.bool:
+        raise ValueError(f"sample_surface: integer face indices, got {faces.dtype}")
+    V = vertices.shape[0]
+    if int(faces.min()) < 0 or int(faces.max()) >= V:
+        raise ValueError(f"sample_surface: face indices outside [0, {V})")
     v = vertices.to(torch.float32).contiguous()
+    if not bool(torch.isfinite(v).all()):
+        raise ValueError("sample_surface: non-finite vertex coordinates")
     f = faces.to(torch.int32).contiguous()
     F = f.shape[0]
     ws = torch.empty(lib().ma_sample_surface_workspace_bytes(F), dtype=torch.uint8, device=v.device)
@@ -206,6 +239,96 @@ def sample_surface(vertices: torch.Tensor, faces: torch.Tensor, n_samples: int, 
     check(lib().ma_sample_surface(ptr(v), ptr(f), F, n_samples, int(seed), ptr(out), ptr(idx), ptr(ws), stream_ptr()),
           "ma_sample_surface")
     return (out, idx) if want_index else out
+
+
+# ---------------------------------------------------------------- glue kernels of the encoder / detokenizer (test hooks)
+
+def fourier_embed_f16(pc: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """pc fp16 [rows, 6] -> fp16 [rows, 256] = [xyz | sin 24 | cos 24 | normal | zeros] (a1 of the encoder)."""
+    _need_cuda(pc, out)
+    assert pc.dtype == torch.float16 and pc.is_contiguous() and pc.dim() == 2 and pc.shape[1] == 6
+    rows = pc.shape[0]
+    if out is None:
+        out = torch.empty((rows, 256), dtype=torch.float16, device=pc.device)
+    assert out.dtype == torch.float16 and out.is_contiguous() and out.numel() >= rows * 256
+    check(lib().ma_fourier_embed_f16(ptr(pc), rows, ptr(out), stream_ptr()), "ma_fourier_embed_f16")
+    return out
+
+
+def scatter_heads_f16(src: torch.Tensor, col0: int, head_stride: int, H: int, rows_per_slot: int, T: int,
+                      dst: torch.Tensor, rows: Optional[int] = None) -> torch.Tensor:
+    """Head slices of src fp16 [rows, ld] into dst (flat fp16, >= (rows / rows_per_slot) * H * T * 64 elements):
+    dst[((slot H + h) T + t) 64 + d] = src[m, col0 + h head_stride + d], slot = m // rows_per_slot,
+    t = m % rows_per_slot."""
+    _need_cuda(src, dst)
+    assert src.dtype == torch.float16 and dst.dtype == torch.float16 and src.stride(1) == 1 and dst.is_contiguous()
+    rows = src.shape[0] if rows is None else rows
+    check(lib().ma_scatter_heads_f16(ptr(src), src.stride(0), col0, head_stride, H, rows_per_slot, T, ptr(dst), rows,
+                                     stream_ptr()), "ma_scatter_heads_f16")
+    return dst
+
+
+def residual_add(x: torch.Tensor, y: torch.Tensor) -> torch.Tensor:
+    """In place: x fp32 += float(y), or x fp16 = fp16(float(x) + float(y)); y fp16, numel % 4 == 0."""
+    _need_cuda(x, y)
+    assert x.is_contiguous() and y.is_contiguous() and y.dtype == torch.float16 and x.numel() == y.numel()
+    x32, x16 = (x, None) if x.dtype == torch.float32 else (None, x)
+    check(lib().ma_residual_add(ptr(x32), ptr(x16), ptr(y), x.numel(), stream_ptr()), "ma_residual_add")
+    return x
+
+
+def convert_rows(src: torch.Tensor, dst: torch.Tensor, rows: int, cols: int, src_rows_mod: int = 0) -> torch.Tensor:
+    """dst[r, :cols] = src[r % src_rows_mod (or r), :cols] converted to dst's dtype (fp16 / fp32); src and dst may be
+    row-strided views: their stride(0) is passed as lds / ldd."""
+    _need_cuda(src, dst)
+    assert src.dtype in (torch.float16, torch.float32) and dst.dtype in (torch.float16, torch.float32)
+    assert src.stride(1) == 1 and dst.stride(1) == 1
+    check(lib().ma_convert_rows(ptr(src), int(src.dtype == torch.float16), src.stride(0), ptr(dst),
+                                int(dst.dtype == torch.float16), dst.stride(0), rows, cols, src_rows_mod, stream_ptr()),
+          "ma_convert_rows")
+    return dst
+
+
+def add_table(y16: torch.Tensor, table: torch.Tensor, mask: Optional[torch.Tensor] = None,
+              out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """fp32 [rows, 768] = (mask[r] ? float(y16[r]) : 0) + table[r % table_rows]."""
+    _need_cuda(y16, table, mask, out)
+    assert y16.dtype == torch.float16 and table.dtype == torch.float32 and y16.is_contiguous() and table.is_contiguous()
+    assert y16.shape[1] == 768 and table.shape[1] == 768 and (mask is None or mask.dtype == torch.int32)
+    if out is None:
+        out = torch.empty((y16.shape[0], 768), dtype=torch.float32, device=y16.device)
+    assert out.dtype == torch.float32 and out.is_contiguous() and out.shape == (y16.shape[0], 768)
+    check(lib().ma_add_table(ptr(y16), ptr(mask), ptr(table), table.shape[0], ptr(out), y16.shape[0], stream_ptr()),
+          "ma_add_table")
+    return out
+
+
+def gather_codes(gen_ids: torch.Tensor, F: int, codebook: torch.Tensor, out=None):
+    """gen_ids int32 [B, max_new] -> (code16 fp16 [B*F, 3072], mask int32 [B*F], ids int32 [B*F, 9]); `out` may give
+    the three destination tensors."""
+    _need_cuda(gen_ids, codebook)
+    assert gen_ids.dtype == torch.int32 and gen_ids.is_contiguous() and codebook.dtype == torch.float32
+    assert codebook.is_contiguous() and codebook.shape[1] == 1024
+    B, max_new = gen_ids.shape
+    dev = gen_ids.device
+    code16, mask, ids = out if out is not None else (
+        torch.empty((B * F, 3072), dtype=torch.float16, device=dev), torch.empty((B * F,), dtype=torch.int32, device=dev),
+        torch.empty((B * F, 9), dtype=torch.int32, device=dev))
+    check(lib().ma_gather_codes(ptr(gen_ids), max_new, B, F, ptr(codebook), ptr(code16), ptr(mask), ptr(ids),
+                                stream_ptr()), "ma_gather_codes")
+    return code16, mask, ids
+
+
+def coords(logits: torch.Tensor, mask: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """logits fp16 [faces, 1152] -> fp32 [faces, 9] = argmax bin / 128 - 0.5 (lowest index on ties), NaN where mask is 0."""
+    _need_cuda(logits, mask, out)
+    assert logits.dtype == torch.float16 and logits.is_contiguous() and logits.shape[1] == 1152
+    assert mask.dtype == torch.int32 and mask.is_contiguous()
+    faces = logits.shape[0]
+    if out is None:
+        out = torch.empty((faces, 9), dtype=torch.float32, device=logits.device)
+    check(lib().ma_coords(ptr(logits), ptr(mask), ptr(out), faces, stream_ptr()), "ma_coords")
+    return out
 
 
 def udf_grid(vertices: torch.Tensor, faces: torch.Tensor, n: int, band: Optional[float] = None) -> torch.Tensor:

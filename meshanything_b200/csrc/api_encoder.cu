@@ -310,6 +310,75 @@ int ma_linear_tc_f16(const void* W, const void* bias, const void* x, int ldx, vo
                           (cudaStream_t)stream);
 }
 
+// ---- test hooks: the glue kernels of glue.cu, one entry point per launcher.  Each refuses what its kernel cannot take
+// (null pointers, non-positive counts, a width or an alignment its vector accesses need) before anything is launched.
+static bool aligned(const void* p, int bytes) { return ((uintptr_t)p & (uintptr_t)(bytes - 1)) == 0; }
+
+int ma_fourier_embed_f16(const void* pc, long rows, void* out, void* stream) {
+  if (!pc || !out || rows <= 0 || !aligned(out, 8)) {
+    set_error("ma_fourier_embed_f16: bad arguments (non-null pointers, rows > 0, out 8-byte aligned)");
+    return 1;
+  }
+  return launch_fourier_embed((const __half*)pc, rows, (__half*)out, (cudaStream_t)stream);
+}
+
+int ma_scatter_heads_f16(const void* src, int ld, int col0, int head_stride, int H, int rows_per_slot, long T, void* dst,
+                         long rows, void* stream) {
+  if (!src || !dst || ld <= 0 || col0 < 0 || head_stride < 0 || H <= 0 || rows_per_slot <= 0 || T <= 0 || rows <= 0 ||
+      ld % 8 || col0 % 8 || head_stride % 8 || !aligned(src, 16) || !aligned(dst, 16)) {
+    set_error("ma_scatter_heads_f16: bad arguments (non-null 16-byte aligned pointers, positive counts, ld, col0 and "
+              "head_stride multiples of 8)");
+    return 1;
+  }
+  return launch_scatter_heads((const __half*)src, ld, col0, head_stride, H, rows_per_slot, T, (__half*)dst, rows,
+                              (cudaStream_t)stream);
+}
+
+int ma_residual_add(float* x32, void* x16, const void* y, long n, void* stream) {
+  if (!y || !x32 == !x16 || n <= 0 || n % 4 || !aligned(y, 8) || !aligned(x32, 16) || !aligned(x16, 8)) {
+    set_error("ma_residual_add: bad arguments (exactly one of x32 / x16, y non-null, n > 0 and n %% 4 == 0, aligned)");
+    return 1;
+  }
+  return launch_residual_add(x32, (__half*)x16, (const __half*)y, n, (cudaStream_t)stream);
+}
+
+int ma_convert_rows(const void* src, int src_f16, long lds, void* dst, int dst_f16, long ldd, long rows, int cols,
+                    long src_rows_mod, void* stream) {
+  if (!src || !dst || lds <= 0 || ldd <= 0 || rows <= 0 || cols <= 0 || cols % 4 || src_rows_mod < 0) {
+    set_error("ma_convert_rows: bad arguments (non-null pointers, positive strides and counts, cols %% 4 == 0, "
+              "src_rows_mod >= 0)");
+    return 1;
+  }
+  return launch_convert_rows(src, src_f16, lds, dst, dst_f16, ldd, rows, cols, src_rows_mod, (cudaStream_t)stream);
+}
+
+int ma_add_table(const void* y16, const int* mask, const float* table, int table_rows, float* out, long rows,
+                 void* stream) {
+  if (!y16 || !table || !out || table_rows <= 0 || rows <= 0 || !aligned(y16, 8) || !aligned(table, 16) ||
+      !aligned(out, 16)) {
+    set_error("ma_add_table: bad arguments (non-null aligned y16 / table / out, positive counts)");
+    return 1;
+  }
+  return launch_add_table((const __half*)y16, mask, table, table_rows, out, rows, (cudaStream_t)stream);
+}
+
+int ma_gather_codes(const int32_t* gen_ids, int max_new, int B, int F, const float* codebook, void* code16, int* mask,
+                    int32_t* ids_out, void* stream) {
+  if (!gen_ids || !codebook || !code16 || !mask || max_new <= 0 || B <= 0 || F <= 0) {
+    set_error("ma_gather_codes: bad arguments (non-null pointers, positive counts)");
+    return 1;
+  }
+  return launch_gather_codes(gen_ids, max_new, B, F, codebook, (__half*)code16, mask, ids_out, (cudaStream_t)stream);
+}
+
+int ma_coords(const void* logits, const int* mask, float* xyz, long faces, void* stream) {
+  if (!logits || !mask || !xyz || faces <= 0) {
+    set_error("ma_coords: bad arguments (non-null pointers, faces > 0)");
+    return 1;
+  }
+  return launch_coords((const __half*)logits, mask, xyz, faces, (cudaStream_t)stream);
+}
+
 size_t ma_encoder_workspace_bytes(int B) { return carve_enc(nullptr, std::min(B, ENC_CHUNK)).total; }
 
 int ma_encoder_forward(const ma_encoder_weights* e, const void* pc_normal, int B, float* point_feature, float* prefix,

@@ -34,27 +34,38 @@ __device__ __forceinline__ float3 sf_philox3(unsigned long long seed, uint32_t i
 
 __device__ __forceinline__ float3 sf_vertex(const float* v, int i) { return make_float3(v[3 * i], v[3 * i + 1], v[3 * i + 2]); }
 
-// area[f] (double: the cumulative sum of up to millions of faces must stay monotone and exact enough for the search)
+// area[f] (double: the cumulative sum of up to millions of faces must stay monotone and exact enough for the search).
+// Here and in surface_sample_kernel every operation carries an explicit rounding, so nvcc contracts nothing and the
+// numpy restatement (tests/surface_oracle.py) reproduces the bits: DESIGN.md section 1.5.
 __global__ void surface_area_kernel(const float* __restrict__ v, const int32_t* __restrict__ faces, int F, double* __restrict__ area) {
   const int f = blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= F) return;
   const float3 a = sf_vertex(v, faces[3 * f]), b = sf_vertex(v, faces[3 * f + 1]), c = sf_vertex(v, faces[3 * f + 2]);
-  const double ux = (double)b.x - a.x, uy = (double)b.y - a.y, uz = (double)b.z - a.z;
-  const double wx = (double)c.x - a.x, wy = (double)c.y - a.y, wz = (double)c.z - a.z;
-  const double nx = uy * wz - uz * wy, ny = uz * wx - ux * wz, nz = ux * wy - uy * wx;
-  area[f] = 0.5 * sqrt(nx * nx + ny * ny + nz * nz);
+  const double ux = __dsub_rn(b.x, a.x), uy = __dsub_rn(b.y, a.y), uz = __dsub_rn(b.z, a.z);
+  const double wx = __dsub_rn(c.x, a.x), wy = __dsub_rn(c.y, a.y), wz = __dsub_rn(c.z, a.z);
+  const double nx = __dsub_rn(__dmul_rn(uy, wz), __dmul_rn(uz, wy));
+  const double ny = __dsub_rn(__dmul_rn(uz, wx), __dmul_rn(ux, wz));
+  const double nz = __dsub_rn(__dmul_rn(ux, wy), __dmul_rn(uy, wx));
+  const double s = __dadd_rn(__dadd_rn(__dmul_rn(nx, nx), __dmul_rn(ny, ny)), __dmul_rn(nz, nz));
+  area[f] = __dmul_rn(0.5, __dsqrt_rn(s));
 }
 
-// in-place inclusive scan by ONE CTA of 1024 threads walking the array in tiles (F is at most a few million)
+// in-place inclusive scan by ONE CTA of 1024 threads walking the array in tiles (F is at most a few million), followed
+// by a running maximum over the faces of positive area.  The Hillis-Steele sums alone are not monotone: two neighbours
+// are summed in different orders, so the cumulative area can step down by an ulp, or up by one across a face of zero
+// area, which the search below would then pick.  The maximum is exact and order-free: cum[i] = max over j <= i with
+// area[j] > 0 of the sum up to j (0 before the first such face).  So cum never decreases, and a face of zero area has
+// cum[i] = cum[i - 1]: it is never drawn.
 __global__ void __launch_bounds__(1024) surface_scan_kernel(double* __restrict__ a, int F) {
-  __shared__ double wsum[32];
-  __shared__ double carry;
+  __shared__ double wsum[32], wmax[32];
+  __shared__ double carry, mcarry;
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (tid == 0) carry = 0.0;
+  if (tid == 0) carry = mcarry = 0.0;
   __syncthreads();
   for (int base = 0; base < F; base += 1024) {
     const int i = base + tid;
-    double x = i < F ? a[i] : 0.0;
+    const double v = i < F ? a[i] : 0.0;
+    double x = v;
 #pragma unroll
     for (int o = 1; o < 32; o <<= 1) {
       const double y = __shfl_up_sync(0xffffffffu, x, o);
@@ -73,9 +84,23 @@ __global__ void __launch_bounds__(1024) surface_scan_kernel(double* __restrict__
     }
     __syncthreads();
     const double off = carry + (warp ? wsum[warp - 1] : 0.0);
-    if (i < F) a[i] = x + off;
+    const double sum = x + off;
+    double m = v > 0.0 ? sum : 0.0;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) m = fmax(m, __shfl_up_sync(0xffffffffu, m, o));  // lanes < o get their own m back
+    if (lane == 31) wmax[warp] = m;
     __syncthreads();
-    if (tid == 1023) carry = x + off;
+    if (warp == 0) {
+      double s = wmax[lane];
+#pragma unroll
+      for (int o = 1; o < 32; o <<= 1) s = fmax(s, __shfl_up_sync(0xffffffffu, s, o));
+      wmax[lane] = s;
+    }
+    __syncthreads();
+    m = fmax(m, fmax(mcarry, warp ? wmax[warp - 1] : 0.0));
+    if (i < F) a[i] = m;
+    __syncthreads();
+    if (tid == 1023) { carry = sum; mcarry = m; }
     __syncthreads();
   }
 }
@@ -95,15 +120,19 @@ __global__ void surface_sample_kernel(const float* __restrict__ v, const int32_t
   const int f = lo;
   const float3 a = sf_vertex(v, faces[3 * f]), b = sf_vertex(v, faces[3 * f + 1]), c = sf_vertex(v, faces[3 * f + 2]);
   float r1 = u.y, r2 = u.z;
-  if (r1 + r2 > 1.0f) { r1 = 1.0f - r1; r2 = 1.0f - r2; }
-  const float ux = b.x - a.x, uy = b.y - a.y, uz = b.z - a.z, wx = c.x - a.x, wy = c.y - a.y, wz = c.z - a.z;
-  const float px = a.x + r1 * ux + r2 * wx, py = a.y + r1 * uy + r2 * wy, pz = a.z + r1 * uz + r2 * wz;
-  float nx = uy * wz - uz * wy, ny = uz * wx - ux * wz, nz = ux * wy - uy * wx;
-  const float ln = sqrtf(nx * nx + ny * ny + nz * nz);
-  const float inv = ln > 0.0f ? 1.0f / ln : 1.0f;
+  if (fadd(r1, r2) > 1.0f) { r1 = fsub(1.0f, r1); r2 = fsub(1.0f, r2); }
+  const float ux = fsub(b.x, a.x), uy = fsub(b.y, a.y), uz = fsub(b.z, a.z);
+  const float wx = fsub(c.x, a.x), wy = fsub(c.y, a.y), wz = fsub(c.z, a.z);
+  const float px = fadd(fadd(a.x, fmul(r1, ux)), fmul(r2, wx));
+  const float py = fadd(fadd(a.y, fmul(r1, uy)), fmul(r2, wy));
+  const float pz = fadd(fadd(a.z, fmul(r1, uz)), fmul(r2, wz));
+  const float nx = fsub(fmul(uy, wz), fmul(uz, wy)), ny = fsub(fmul(uz, wx), fmul(ux, wz));
+  const float nz = fsub(fmul(ux, wy), fmul(uy, wx));
+  const float ln = __fsqrt_rn(fadd(fadd(fmul(nx, nx), fmul(ny, ny)), fmul(nz, nz)));
+  const float inv = ln > 0.0f ? __fdiv_rn(1.0f, ln) : 1.0f;
   __half* o = out + (size_t)i * 6;
   o[0] = __float2half_rn(px); o[1] = __float2half_rn(py); o[2] = __float2half_rn(pz);
-  o[3] = __float2half_rn(nx * inv); o[4] = __float2half_rn(ny * inv); o[5] = __float2half_rn(nz * inv);
+  o[3] = __float2half_rn(fmul(nx, inv)); o[4] = __float2half_rn(fmul(ny, inv)); o[5] = __float2half_rn(fmul(nz, inv));
   if (face_idx) face_idx[i] = f;
 }
 

@@ -91,6 +91,41 @@ def test_attention_bit_exact(H, T, nk):
 
 
 @gpu
+def test_attention_at_the_encoder_layout_on_one_scratch():
+    """The encoder's use of the canonical attention: 8 shapes x 257 latent rows, 12 heads, slot = row // 257, first over
+    the 4096 point keys (16 chunks) and then over 257 keys (2 chunks), both launches on ONE scratch area zeroed once --
+    the kernel re-arms its per-(row, head) counters itself.  Sampled rows bit for bit against the oracle."""
+    import ctypes
+    from meshanything_b200 import capi
+    from oracle import decoder as orc
+    d = _dev()
+    L = capi.lib()
+    S, R, H = 8, 257, 12
+    M = S * R
+    scratch = torch.zeros(L.ma_attention_scratch_bytes(M, H, 4096), dtype=torch.uint8, device=d)
+    slots = (torch.arange(M, dtype=torch.int32) // R).to(d)
+    g = torch.Generator().manual_seed(257)
+    rows = sorted(set([s * R for s in range(S)] + [s * R + R - 1 for s in range(S)]
+                      + torch.randperm(M, generator=g)[:64].tolist()))
+    for T in (4096, 257):
+        q = torch.randn(M, H, 64, generator=g).half()
+        k = torch.randn(S, H, T, 64, generator=g).half()
+        v = torch.randn(S, H, T, 64, generator=g).half()
+        qd, kd, vd = q.to(d), k.to(d), v.to(d)
+        nkeys = torch.full((M,), T, dtype=torch.int32, device=d)
+        out = torch.empty((M, H, 64), dtype=torch.float16, device=d)
+        capi.check(L.ma_attention_f16(capi.ptr(qd), H * 64, capi.ptr(kd), capi.ptr(vd), T, H,
+                                      capi.ptr(slots), capi.ptr(nkeys), T, M, ctypes.c_float(0.125), capi.ptr(out),
+                                      H * 64, capi.ptr(scratch), capi.stream_ptr()), "ma_attention_f16")
+        torch.cuda.synchronize()
+        out = out.cpu()
+        for s in range(S):
+            mine = [m for m in rows if m // R == s]
+            ref = orc.attention(q[mine], k[s], v[s], [T] * len(mine))
+            assert torch.equal(out[mine].view(torch.int16), ref.view(torch.int16)), (T, s)
+
+
+@gpu
 @pytest.mark.parametrize("T,nk", [(300, [1, 2, 33, 256, 257, 258, 300]), (1100, [1100, 513, 1024, 1025, 7]),
                                   (7500, [7459, 7425, 258, 4096] * 6)])
 def test_attention_decode_stream_bit_exact(T, nk):

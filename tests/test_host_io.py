@@ -9,6 +9,17 @@ CUBE = """v 0 0 0\nv 1 0 0\nv 1 1 0\nv 0 1 0\nv 0 0 1\nv 1 0 1\nv 1 1 1\nv 0 1 1
 f 1 2 3 4\nf 5 8 7 6\nf 1 5 6 2\nf 2 6 7 3\nf 3 7 8 4\nf 5 1 4 8\n"""
 
 
+@pytest.mark.parametrize("face", ["f 1 2 9", "f 0 1 2", "f 1 2 -9"])
+def test_obj_face_outside_the_vertex_list_raises(tmp_path, face):
+    """A face index past the vertices read so far (or 0, or a relative index before the first) is refused at load time
+    instead of reaching the surface sampler."""
+    import mesh_to_pc
+    p = tmp_path / "bad.obj"
+    p.write_text(CUBE + face + "\n")
+    with pytest.raises(ValueError, match="outside 1..8"):
+        mesh_to_pc.SimpleMesh.load_obj(str(p))
+
+
 def test_numpy_mesh_sampler(tmp_path):
     import mesh_to_pc
     p = tmp_path / "cube.obj"
