@@ -402,6 +402,31 @@ int ma_farthest_point_sample(const float* xyz, int n, int m, int start, int64_t*
 int ma_farthest_point_sample_set_path(int path);
 int ma_farthest_point_sample_last_path(void);
 
+/* ---- removal of the dominant plane of a point cloud (`--remove_plane`; csrc/plane.cu) ------------------------------
+ * xyz fp32 [n][3], finite, already in the output frame -> what DESIGN.md section 1.6 keeps: h RANSAC hypotheses, each the
+ * fp32 plane (n, d) through three points drawn by Philox4x32-10 (counter (h, "PLAN", "MESH", "ANYT"), key = seed) --
+ * invalid, stored as (0, 0, 0, +inf) and scoring 0, when the cross product is zero or not finite; a point is on a
+ * plane iff |((nx px + ny py) + nz pz) + d| <= t in fp32 without contraction; the winner has the most on-plane points
+ * (lowest h on ties), and no plane is found when that count is below 3.  The winner's on-plane points are refitted
+ * (fixed-order fp64 centroid and second moments, the Jacobi of section 1.2), every point is classified on / above /
+ * below the refit plane, the plane is flipped when below > above, and the points above it are kept.
+ * Device outputs: keep_out uint8 [n] (1 = kept), kept_idx_out int64 [n] (the first *n_kept_out entries: the kept
+ * indices, ascending), n_kept_out int64 [1], stats_out fp64 [12] = (found, nx, ny, nz, d of the refit plane after the
+ * flip (zeros when nothing is found), winning hypothesis, its count, valid hypotheses, on, above, below (zeros when
+ * nothing is found), kept points).  Optional (NULL: not written): counts_out int32 [h] (on-plane points of every
+ * hypothesis), planes_out fp32 [h][4] (every hypothesis's (nx, ny, nz, d)).
+ * 3 <= n <= 2^24, 1 <= h <= 65536, 0 < t <= 1, any 64-bit seed.  ws: ma_remove_plane_workspace_bytes(n, h) bytes (no
+ * device needed; 0 for shapes out of range).  No host synchronisation and no floating-point atomics: two calls give
+ * identical bits. */
+size_t ma_remove_plane_workspace_bytes(int n, int h);
+int ma_remove_plane(const float* xyz, int n, int h, float t, unsigned long long seed, uint8_t* keep_out,
+                    int64_t* kept_idx_out, int64_t* n_kept_out, int32_t* counts_out, float* planes_out,
+                    double* stats_out, void* ws, void* stream);
+/* Measurement hook (tools/bench_plane.py): events = 5 cudaEvent_t recorded on the stream of every following call at
+ * its start and after the hypotheses, the scoring (with the winner), the refit and the classification with the
+ * compaction (NULL: off). */
+void ma_remove_plane_set_events(void* const* events);
+
 /* number of kernels launched by the library since load (bench.py's gpu_launches) */
 unsigned long long ma_launch_count(void);
 

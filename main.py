@@ -4,6 +4,7 @@
     python main.py --input_type pc --input_path scan.npy       # bare (N, 3) cloud: normals estimated on the GPU
     python main.py --input_type pc --input_path scan.npy --remove_outliers   # drop stray points / floaters first
     python main.py --input_type pc --input_path scan.npy --subsample fps     # even coverage of uneven scan density
+    python main.py --input_type pc --input_path scan.npy --remove_plane      # drop the table / floor under the object
     torchrun --nproc-per-node 8 main.py --input_type pc_normal --input_dir pcs --batchsize_per_gpu 64
 
 Differences forced by the environment: no accelerate / hf_hub (there is no network) -- one process per
@@ -37,6 +38,26 @@ def _remove_outliers(xyz, path, outliers, n_points=4096):
     return idx.cpu().numpy()
 
 
+def _remove_plane(xyz, path, plane, n_points=4096):
+    """`--remove_plane`: the indices of the points of xyz [N, 3] that DESIGN.md section 1.6 keeps (on the GPU,
+    meshanything_b200.plane): the dominant plane and everything below it go.  The RANSAC seed is drawn from the global
+    numpy RNG, so --seed selects it; one line per input with the plane and the counts."""
+    from meshanything_b200.plane import remove_plane
+    seed = int(np.random.randint(0, 2**62, dtype=np.int64))
+    idx, st = remove_plane(xyz, seed=seed, **plane)
+    if st.found:
+        n = st.normal
+        print(f"{_uid_of(path)}: plane n = ({n[0]:.4f}, {n[1]:.4f}, {n[2]:.4f}), d = {st.offset:.4f} (output frame), "
+              f"t = {st.threshold:.4g} in input units; removed {st.on} on it and {st.below} below it; {st.kept} of "
+              f"{xyz.shape[0]} kept")
+    else:
+        print(f"{_uid_of(path)}: no plane found ({st.valid_hypotheses} valid hypotheses); {st.kept} points kept")
+    if st.kept < n_points:
+        raise ValueError(f"{path}: {st.kept} points remain after plane removal ({st.on} on the plane, {st.below} below "
+                         f"it), fewer than the {n_points} the model takes")
+    return idx.cpu().numpy()
+
+
 def _farthest_points(xyz, path, n_points=4096):
     """`--subsample fps`: the picks of farthest-point sampling (DESIGN.md section 1.4, on the GPU,
     meshanything_b200.subsample) from a start drawn from the global numpy RNG, so --seed still selects the subset; one
@@ -49,12 +70,15 @@ def _farthest_points(xyz, path, n_points=4096):
     return idx.cpu().numpy()
 
 
-def _subsample_points(path, n_points=4096, outliers=None, subsample='random'):
+def _subsample_points(path, n_points=4096, outliers=None, subsample='random', plane=None):
     """`--input_type pc_normal`: an .npy of >= 4096 (xyz, normal) rows; a random 4096-subset without replacement
     (global numpy RNG, seeded by --seed as the reference does through accelerate.set_seed), or with
     subsample='fps' the farthest-point subset of the xyz columns.  With `outliers` (the keyword arguments of
-    meshanything_b200.outliers.remove_outliers) the rows are first cleaned by their xyz."""
+    meshanything_b200.outliers.remove_outliers) the rows are first cleaned by their xyz; with `plane` (the keyword
+    arguments of meshanything_b200.plane.remove_plane) the support plane goes before that."""
     cloud = np.load(path)
+    if plane is not None:
+        cloud = cloud[_remove_plane(cloud[:, :3], path, plane, n_points)]
     if outliers is not None:
         cloud = cloud[_remove_outliers(cloud[:, :3], path, outliers, n_points)]
     assert cloud.shape[0] >= n_points, "input pc_normal should have at least 4096 points"
@@ -64,17 +88,20 @@ def _subsample_points(path, n_points=4096, outliers=None, subsample='random'):
     return cloud[keep]
 
 
-def _points_with_normals(path, n_points=4096, k=16, outliers=None, subsample='random'):
+def _points_with_normals(path, n_points=4096, k=16, outliers=None, subsample='random', plane=None):
     """`--input_type pc`: a bare cloud (.npy (N, 3) or vertex-only .ply) of >= 4096 points.  Normals are estimated on
     the GPU from all N points (meshanything_b200.normals), then the same 4096-subset as `pc_normal` is drawn: the
     xyz-only copy of a file selects the points the file with normals selects under the same seed.  With `outliers`
-    the cloud is cleaned first, and normals and subset come from the kept points."""
+    the cloud is cleaned first, and normals and subset come from the kept points; `plane` removes the support plane
+    before that."""
     from mesh_to_pc import load_points
     from meshanything_b200.normals import estimate_normals
     xyz = load_points(path)
     if not np.issubdtype(xyz.dtype, np.floating):
         xyz = xyz.astype(np.float64)
     assert xyz.shape[0] >= n_points, "input pc_normal should have at least 4096 points"
+    if plane is not None:
+        xyz = xyz[_remove_plane(xyz, path, plane, n_points)]
     if outliers is not None:
         xyz = xyz[_remove_outliers(xyz, path, outliers, n_points)]
     normals = estimate_normals(xyz, k).cpu().numpy()
@@ -93,6 +120,8 @@ _NO_MESH_OUTLIERS = ("--remove_outliers applies to point-cloud input (--input_ty
                      "mesh are sampled from its surface and have no outliers")
 _NO_MESH_FPS = ("--subsample fps applies to point-cloud input (--input_type pc or pc_normal): the points of a mesh are "
                 "already sampled uniformly by area")
+_NO_MESH_PLANE = ("--remove_plane applies to point-cloud input (--input_type pc or pc_normal): the points of a mesh are "
+                  "sampled from its own surface, which has no scanned support under it")
 SUBSAMPLERS = ('random', 'fps')
 
 
@@ -108,16 +137,19 @@ class Dataset:
     coordinates centred on the bounding box and scaled to max |x| = 0.9995, unit normals asserted.  `outliers` (point
     clouds only): None, or the keyword arguments of meshanything_b200.outliers.remove_outliers, to clean every cloud
     before normals and subset.  `subsample` (point clouds only): 'random' (the reference's np.random.choice) or 'fps'
-    (farthest-point sampling on the GPU, DESIGN.md section 1.4)."""
+    (farthest-point sampling on the GPU, DESIGN.md section 1.4).  `plane` (point clouds only): None, or the keyword
+    arguments of meshanything_b200.plane.remove_plane, to remove the support plane (a table, the floor) first."""
 
-    def __init__(self, input_type, input_list, mc=False, outliers=None, subsample='random'):
+    def __init__(self, input_type, input_list, mc=False, outliers=None, subsample='random', plane=None):
         if outliers is not None and input_type not in ('pc', 'pc_normal'):
             raise ValueError(_NO_MESH_OUTLIERS)
+        if plane is not None and input_type not in ('pc', 'pc_normal'):
+            raise ValueError(_NO_MESH_PLANE)
         _check_subsample(input_type, subsample)
         if input_type == 'pc_normal':
-            clouds = [_subsample_points(p, outliers=outliers, subsample=subsample) for p in input_list]
+            clouds = [_subsample_points(p, outliers=outliers, subsample=subsample, plane=plane) for p in input_list]
         elif input_type == 'pc':
-            clouds = [_points_with_normals(p, outliers=outliers, subsample=subsample) for p in input_list]
+            clouds = [_points_with_normals(p, outliers=outliers, subsample=subsample, plane=plane) for p in input_list]
         elif input_type == 'mesh':
             if mc:
                 print("First Marching Cubes and then sample point cloud, need several minutes...")
@@ -169,6 +201,11 @@ def get_args():
     # reference's np.random.choice) or 'fps', farthest-point sampling on the GPU, which covers a scan evenly whatever
     # its density (DESIGN.md section 1.4; meshanything_b200.subsample)
     parser.add_argument('--subsample', default='random', choices=SUBSAMPLERS)
+    # not in the reference: remove the plane a scanned object stands on (a table, a turntable, the floor) and
+    # everything below it, by RANSAC and a least-squares refit on the GPU (DESIGN.md section 1.6; meshanything_b200.plane)
+    parser.add_argument('--remove_plane', default=False, action="store_true")
+    parser.add_argument('--plane_distance', default=0.01, type=float)
+    parser.add_argument('--plane_iterations', default=1000, type=int)
     return parser.parse_args()
 
 
@@ -178,6 +215,13 @@ def outlier_options(args):
         return None
     return {'k': args.outlier_neighbors, 'std_ratio': args.outlier_std_ratio,
             'min_component': args.outlier_min_component}
+
+
+def plane_options(args):
+    """The `plane` argument of Dataset from the command line: None without --remove_plane."""
+    if not getattr(args, 'remove_plane', False):
+        return None
+    return {'distance': getattr(args, 'plane_distance', 0.01), 'iterations': getattr(args, 'plane_iterations', 1000)}
 
 
 def check_args(args):
@@ -197,6 +241,16 @@ def check_args(args):
                 and args.outlier_min_component >= 0):
             raise ValueError("--outlier_std_ratio must be finite and --outlier_min_component finite and >= 0")
     _check_subsample(args.input_type, getattr(args, 'subsample', 'random'))   # namespaces built without the flag
+    if getattr(args, 'remove_plane', False):
+        if args.input_type == 'mesh':
+            raise ValueError(_NO_MESH_PLANE)
+        distance = getattr(args, 'plane_distance', 0.01)
+        iterations = getattr(args, 'plane_iterations', 1000)
+        if not (np.isfinite(distance) and 0 < distance <= 1 and np.float32(distance) > 0):
+            raise ValueError(f"--plane_distance must be in (0, 1] (a share of the bounding box's longest side), got "
+                             f"{distance}")
+        if not 1 <= iterations <= 65536:
+            raise ValueError(f"--plane_iterations must be in 1..65536, got {iterations}")
 
 
 def load_model(args, device=None):
@@ -320,7 +374,8 @@ if __name__ == "__main__":
         raise ValueError("input_dir or input_path must be provided.")
     np.random.seed(args.seed)
     torch.manual_seed(args.seed)
-    dataset = Dataset(args.input_type, input_list, args.mc, outliers=outlier_options(args), subsample=args.subsample)
+    dataset = Dataset(args.input_type, input_list, args.mc, outliers=outlier_options(args), subsample=args.subsample,
+                      plane=plane_options(args))
 
     bs = args.batchsize_per_gpu
     batches = [list(range(i, min(i + bs, len(dataset)))) for i in range(0, len(dataset), bs)]

@@ -53,6 +53,7 @@ EXPORTS = [
     "ma_remove_outliers_workspace_bytes", "ma_remove_outliers", "ma_remove_outliers_set_events",
     "ma_farthest_point_sample_workspace_bytes", "ma_farthest_point_sample", "ma_farthest_point_sample_set_path",
     "ma_farthest_point_sample_last_path",
+    "ma_remove_plane_workspace_bytes", "ma_remove_plane", "ma_remove_plane_set_events",
     "ma_fourier_embed_f16", "ma_scatter_heads_f16", "ma_residual_add", "ma_convert_rows", "ma_add_table",
     "ma_gather_codes", "ma_coords",
 ]
@@ -149,6 +150,12 @@ def lib():
     L.ma_farthest_point_sample_set_path.restype = C.c_int
     L.ma_farthest_point_sample_last_path.argtypes = []
     L.ma_farthest_point_sample_last_path.restype = C.c_int
+    L.ma_remove_plane_workspace_bytes.argtypes = [C.c_int, C.c_int]
+    L.ma_remove_plane_workspace_bytes.restype = C.c_size_t
+    L.ma_remove_plane.argtypes = [_vp, C.c_int, C.c_int, C.c_float, C.c_ulonglong, _vp, _vp, _vp, _vp, _vp, _vp, _vp,
+                                  _vp]
+    L.ma_remove_plane_set_events.argtypes = [_vp]
+    L.ma_remove_plane_set_events.restype = None
     L.ma_fourier_embed_f16.argtypes = [_vp, C.c_long, _vp, _vp]
     L.ma_scatter_heads_f16.argtypes = [_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_long, _vp, C.c_long, _vp]
     L.ma_residual_add.argtypes = [_vp, _vp, _vp, C.c_long, _vp]
@@ -507,6 +514,69 @@ def farthest_point_sample(points: torch.Tensor, m: int, start: int = 0):
         check(lib().ma_farthest_point_sample(ptr(points), n, m, start, ptr(idx), ptr(r2), ptr(ws), stream_ptr()),
               "ma_farthest_point_sample")
     return idx, r2
+
+
+PLANE_MAX_H = 65536
+
+
+def remove_plane(points: torch.Tensor, distance: float = 0.01, iterations: int = 1000, seed: int = 0,
+                 want_terms: bool = False):
+    """Removal of the dominant plane of a cloud (ma_remove_plane; plane.remove_plane adds the frame map).
+
+    points fp32 [N, 3], contiguous, on a CUDA device, finite, already in the output frame; 3 <= N <= 2^24; distance the
+    on-plane threshold t in the frame, 0 < t <= 1 (rounded to fp32, which must stay > 0); 1 <= iterations <= 65536
+    hypotheses; an integer seed in [0, 2^64).  Returns (kept indices int64 [n_kept] ascending, keep mask bool [N],
+    stats fp64 [12] on the host: found, nx, ny, nz, d, winning hypothesis, its count, valid hypotheses, on, above,
+    below, kept); with want_terms also (on-plane count int32 [H] and plane fp32 [H, 4] of every hypothesis).  Every bad
+    input raises ValueError before anything is launched.  Reads the stats back (synchronises)."""
+    if not isinstance(points, torch.Tensor):
+        raise ValueError(f"remove_plane: points must be a torch tensor, got {type(points).__name__}")
+    if points.dim() != 2 or points.shape[1] != 3:
+        raise ValueError(f"remove_plane: points [N, 3], got {tuple(points.shape)}")
+    if points.dtype != torch.float32:
+        raise ValueError(f"remove_plane: points must be float32, got {points.dtype}")
+    if not points.is_contiguous():
+        raise ValueError("remove_plane: points must be contiguous")
+    if not points.is_cuda:
+        raise ValueError("remove_plane: points must live on a CUDA device (no CPU fallback)")
+    n = points.shape[0]
+    if not 3 <= n <= 1 << 24:
+        raise ValueError(f"remove_plane: 3 <= N <= 2^24, got N = {n}")
+    if isinstance(iterations, bool) or isinstance(seed, bool):
+        raise ValueError("remove_plane: iterations and seed must be integers")
+    try:
+        iterations, seed = operator.index(iterations), operator.index(seed)
+    except TypeError:
+        raise ValueError(f"remove_plane: iterations and seed must be integers, got {iterations!r}, {seed!r}") from None
+    if not 1 <= iterations <= PLANE_MAX_H:
+        raise ValueError(f"remove_plane: 1 <= iterations <= {PLANE_MAX_H}, got {iterations}")
+    if not 0 <= seed < 1 << 64:
+        raise ValueError(f"remove_plane: 0 <= seed < 2^64, got {seed}")
+    if isinstance(distance, bool):
+        raise ValueError("remove_plane: distance must be a real number")
+    try:
+        distance = float(distance)
+    except (TypeError, ValueError):
+        raise ValueError(f"remove_plane: distance must be a real number, got {distance!r}") from None
+    t32 = C.c_float(distance).value
+    if not (math.isfinite(distance) and 0 < distance <= 1 and 0 < t32 <= 1):
+        raise ValueError(f"remove_plane: 0 < distance <= 1 (and > 0 in fp32), got {distance}")
+    if not bool(torch.isfinite(points).all()):
+        raise ValueError("remove_plane: non-finite coordinates")
+    dev = points.device
+    ws = torch.empty(lib().ma_remove_plane_workspace_bytes(n, iterations), dtype=torch.uint8, device=dev)
+    keep = torch.empty((n,), dtype=torch.uint8, device=dev)
+    idx = torch.empty((n,), dtype=torch.int64, device=dev)
+    n_kept = torch.empty((1,), dtype=torch.int64, device=dev)
+    stats = torch.empty((12,), dtype=torch.float64, device=dev)
+    counts = torch.empty((iterations,), dtype=torch.int32, device=dev) if want_terms else None
+    planes = torch.empty((iterations, 4), dtype=torch.float32, device=dev) if want_terms else None
+    with torch.cuda.device(dev):
+        check(lib().ma_remove_plane(ptr(points), n, iterations, C.c_float(t32), seed, ptr(keep), ptr(idx), ptr(n_kept),
+                                    ptr(counts), ptr(planes), ptr(stats), ptr(ws), stream_ptr()), "ma_remove_plane")
+        st = stats.cpu().numpy()
+    out = (idx[:int(st[11])], keep.bool(), st)
+    return (*out, counts, planes) if want_terms else out
 
 
 def tensor_core_linear_counts():

@@ -6,8 +6,8 @@
 //   (b) kNN       knn_grid_kernel (knn_grid.cuh), one thread per point, shells of cells until the k-th key's d^2 is
 //                 below the bound of the next shell, without a shell budget: the exact kNN.
 //   (c) PCA       normals_pca_kernel, one thread per point: fp64 centroid and covariance of the point and its
-//                 neighbours in rank order, sequential sums of explicit __d*_rn operations, then kNmSweeps cyclic
-//                 Jacobi sweeps; the eigenvector of the smallest diagonal entry, normalised in fp64, rounded to fp32.
+//                 neighbours in rank order, sequential sums of explicit __d*_rn operations, then the cyclic Jacobi
+//                 of jacobi3.cuh; the eigenvector of the smallest diagonal entry, normalised in fp64, rounded to fp32.
 //   (d) orient    Boruvka over the kNN graph.  Each vertex carries a word (component root << 1 | parity), the parity
 //                 being its sign relative to that root.  A round: every component's minimum outgoing edge under the
 //                 strict order (w, min(i,j), max(i,j)) by two 64/32-bit atomicMin passes over unique keys; each
@@ -23,12 +23,12 @@
 
 #include "canon.cuh"
 #include "internal.h"
+#include "jacobi3.cuh"
 #include "knn_grid.cuh"
 
 namespace ma {
 
 constexpr int kNmThreads = 256;
-constexpr int kNmSweeps = 5;        // Jacobi sweeps: 4 reach 4e-15 rad against LAPACK on separated spectra, 1 spare
 constexpr int kNmMaxN = 1 << 24;    // vertex words hold the root in 31 bits; the index part of a kNN key in 32
 constexpr int kNmMaxRounds = 64;    // Boruvka at least halves the components with an outgoing edge per round
 
@@ -73,44 +73,12 @@ __global__ void normals_pca_kernel(const float* __restrict__ xyz, const int32_t*
       for (int a = 0; a < 6; a++) c[a] = __dadd_rn(c[a], t[a]);
     }
   }
-  double A[3][3] = {{c[0], c[1], c[2]}, {c[1], c[3], c[4]}, {c[2], c[4], c[5]}};
-  double V[3][3] = {{1.0, 0.0, 0.0}, {0.0, 1.0, 0.0}, {0.0, 0.0, 1.0}};
-  for (int sweep = 0; sweep < kNmSweeps; sweep++) {
-#pragma unroll
-    for (int pr = 0; pr < 3; pr++) {
-      const int p = pr == 2 ? 1 : 0, q = pr == 0 ? 1 : 2, r = 2 - pr;
-      const double apq = A[p][q];
-      if (apq == 0.0) continue;
-      const double app = A[p][p], aqq = A[q][q];
-      const double theta = __ddiv_rn(__dsub_rn(aqq, app), __dmul_rn(2.0, apq));
-      double t = __ddiv_rn(1.0, __dadd_rn(fabs(theta), __dsqrt_rn(__dadd_rn(__dmul_rn(theta, theta), 1.0))));
-      if (theta < 0.0) t = -t;
-      const double cs = __ddiv_rn(1.0, __dsqrt_rn(__dadd_rn(__dmul_rn(t, t), 1.0)));
-      const double sn = __dmul_rn(t, cs);
-      const double tapq = __dmul_rn(t, apq);
-      const double arp = A[r][p], arq = A[r][q];
-      A[p][p] = __dsub_rn(app, tapq);
-      A[q][q] = __dadd_rn(aqq, tapq);
-      A[p][q] = A[q][p] = 0.0;
-      A[r][p] = A[p][r] = __dsub_rn(__dmul_rn(cs, arp), __dmul_rn(sn, arq));
-      A[r][q] = A[q][r] = __dadd_rn(__dmul_rn(sn, arp), __dmul_rn(cs, arq));
-#pragma unroll
-      for (int row = 0; row < 3; row++) {
-        const double vp = V[row][p], vq = V[row][q];
-        V[row][p] = __dsub_rn(__dmul_rn(cs, vp), __dmul_rn(sn, vq));
-        V[row][q] = __dadd_rn(__dmul_rn(sn, vp), __dmul_rn(cs, vq));
-      }
-    }
-  }
-  // the column of the smallest diagonal entry, the lowest column on ties
-  double v0 = V[0][0], v1 = V[1][0], v2 = V[2][0], dmin = A[0][0];
-  if (A[1][1] < dmin) { v0 = V[0][1]; v1 = V[1][1]; v2 = V[2][1]; dmin = A[1][1]; }
-  if (A[2][2] < dmin) { v0 = V[0][2]; v1 = V[1][2]; v2 = V[2][2]; }
-  const double ln = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(v0, v0), __dmul_rn(v1, v1)), __dmul_rn(v2, v2)));
+  double v[3];
+  jacobi3_smallest(c, v);
   float* o = uno + 3 * (size_t)i;
-  o[0] = (float)__ddiv_rn(v0, ln);
-  o[1] = (float)__ddiv_rn(v1, ln);
-  o[2] = (float)__ddiv_rn(v2, ln);
+  o[0] = (float)v[0];
+  o[1] = (float)v[1];
+  o[2] = (float)v[2];
 }
 
 // ---------------------------------------------------------------- (d) orientation

@@ -8,28 +8,15 @@
 // (seed, sample), not numpy's Mersenne twister: same distribution, different individual points.
 #include "canon.cuh"
 #include "internal.h"
+#include "philox.cuh"
 
 namespace ma {
 
-__device__ __forceinline__ uint32_t sf_mulhilo(uint32_t a, uint32_t b, uint32_t* hi) {
-  const unsigned long long p = (unsigned long long)a * b;
-  *hi = (uint32_t)(p >> 32);
-  return (uint32_t)p;
-}
 // three uniforms in [0,1) for sample i
 __device__ __forceinline__ float3 sf_philox3(unsigned long long seed, uint32_t i) {
-  uint32_t c0 = i, c1 = 0x53555246u, c2 = 0x4d455348u, c3 = 0x414e5954u;
-  uint32_t k0 = (uint32_t)seed, k1 = (uint32_t)(seed >> 32);
-#pragma unroll
-  for (int r = 0; r < 10; r++) {
-    uint32_t hi0, hi1;
-    const uint32_t lo0 = sf_mulhilo(0xD2511F53u, c0, &hi0), lo1 = sf_mulhilo(0xCD9E8D57u, c2, &hi1);
-    const uint32_t n0 = hi1 ^ c1 ^ k0, n1 = lo1, n2 = hi0 ^ c3 ^ k1, n3 = lo0;
-    c0 = n0; c1 = n1; c2 = n2; c3 = n3;
-    k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
-  }
+  const uint4 c = philox4x32_10(i, 0x53555246u, 0x4d455348u, 0x414e5954u, seed);
   const float s = 1.0f / 16777216.0f;
-  return make_float3((float)(c0 >> 8) * s, (float)(c1 >> 8) * s, (float)(c2 >> 8) * s);
+  return make_float3((float)(c.x >> 8) * s, (float)(c.y >> 8) * s, (float)(c.z >> 8) * s);
 }
 
 __device__ __forceinline__ float3 sf_vertex(const float* v, int i) { return make_float3(v[3 * i], v[3 * i + 1], v[3 * i + 2]); }
