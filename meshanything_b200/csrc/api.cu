@@ -94,12 +94,14 @@ static inline __half* kv_layer(void* kv, int layer, int which, int B, long T) {
   return (__half*)kv + ((size_t)(layer * 2 + which) * B) * NHEAD * T * HD;
 }
 
-// MA_B200_NO_STREAM_ATTN=1: decode steps of a batch use kv_append_kernel + attention_kernel (one CTA per chunk) instead
-// of attention_stream_kernel -- same bits, kept for A/B timing (tools/bench_batched.py)
+// MA_B200_NO_STREAM_ATTN=1: decode steps (of a batch, and at batch 1) use kv_append_kernel + attention_kernel (one CTA
+// per chunk) instead of attention_stream_kernel -- same bits, kept for A/B timing (tools/bench_batched.py,
+// tools/bench_decode_b1.py)
 static const bool g_no_stream_attn = [] {
   const char* e = getenv("MA_B200_NO_STREAM_ATTN");
   return e && e[0] == '1';
 }();
+bool no_stream_attn() { return g_no_stream_attn; }
 
 static const bool g_no_pdl = [] {   // MA_B200_NO_PDL=1: plain stream order between the kernels of a batched decode step
   const char* e = getenv("MA_B200_NO_PDL");

@@ -11,9 +11,13 @@
 //   * activations never leave L2: residual add + LayerNorm are recomputed by every CTA in its
 //     prologue (4 KB read), block 0 publishes the fp32 residual stream;
 //   * dot products follow the canonical order (lane l owns k = 256g + 8l + j; butterfly), identical
-//     to gemm_canon.cu and to the oracle, so batch-1 tokens equal batched tokens bit for bit.
-// Kernels that read data produced two kernels earlier in their PDL prologue (the attention kernel:
-// nkeys, old KV rows) are only ever preceded by a kernel that triggers AFTER its own wait (qkv).
+//     to gemm_canon.cu and to the oracle, so batch-1 tokens equal batched tokens bit for bit;
+//   * attention runs on attention_stream_kernel (M = 1: one CTA per SM, attention_stream.cu), which also appends the
+//     current token's k / v to the cache; qkv writes q | k | v to one buffer.
+// Kernels that read data produced two kernels earlier in their PDL prologue (the attention producer warp: nkeys, old KV
+// rows) are only ever preceded by a kernel that triggers AFTER its own wait (qkv), so every earlier kernel has
+// finished by the time they start.  Under MA_B200_NO_STREAM_ATTN=1 the attention is kv_append_kernel (launched in
+// plain stream order) + attention_kernel, which fetches the old rows early for the same reason.
 #include "canon.cuh"
 #include "internal.h"
 
@@ -31,7 +35,7 @@ enum { MODE_QKV = 0, MODE_OUT = 1, MODE_FC1 = 2, MODE_FC2 = 3, MODE_LM = 4 };
 struct FastWs {  // device-resident scratch of the fast path (inside the decoder workspace)
   float hresA[HID];   // residual stream entering the layer (post-LN2 of the previous layer / embedding)
   float hresB[HID];   // post-LN1 residual stream
-  __half q[HID];
+  __half qkv[QKV];    // q | k | v of the current token
   __half attn16[HID];
   __half y16[HID];
   __half f16[FFN];
@@ -59,8 +63,6 @@ struct FastArgs {
   SeqState s;
   // outputs
   __half* out16;
-  __half *kc, *vc;
-  long T;
   // lm_head
   FastWs* ws;
   int do_argmax;
@@ -178,8 +180,6 @@ __global__ void __launch_bounds__(FG_THREADS) fast_gemv_kernel(FastArgs a) {
 #pragma unroll
   for (int g = 0; g < G; g++) xp[g] = *reinterpret_cast<const uint4*>(sh.xs + 256 * g + 8 * lane);
 
-  int pos = 0;
-  if (MODE == MODE_QKV) pos = a.s.pos[0];
   float bestv = -INFINITY;
   int besti = 0x7fffffff;
 
@@ -211,17 +211,7 @@ __global__ void __launch_bounds__(FG_THREADS) fast_gemv_kernel(FastArgs a) {
         const float bf = a.bias ? __half2float(sb[wr0 + r0 + i]) : 0.0f;
         __half h = __float2half_rn(fadd(sum, bf));
         if (MODE == MODE_FC1 && __half2float(h) < 0.0f) h = __float2half_rn(0.0f);
-        if (MODE == MODE_QKV) {
-          if (n < HID) {
-            a.out16[n] = h;
-          } else {
-            const int e = (n - HID) & (HID - 1), head = e >> 6, d = e & 63;
-            __half* c = (n < 2 * HID) ? a.kc : a.vc;
-            c[((long)head * a.T + pos) * HD + d] = h;
-          }
-        } else {
-          a.out16[n] = h;
-        }
+        a.out16[n] = h;
         if (MODE == MODE_LM) {
           const float v = __half2float(h);
           if (v > bestv || (v == bestv && n < besti)) { bestv = v; besti = n; }
@@ -341,7 +331,6 @@ int fast_step_enqueue(const ma_decoder_weights* w, SeqState s, int tmax, int max
   FastArgs base;
   memset(&base, 0, sizeof(base));
   base.s = s;
-  base.T = T;
   base.ws = ws;
   base.extra = w->extra; base.tok_pos = w->tok_pos; base.cond = w->cond; base.pos_table = w->pos;
   base.tok_table = (const __half*)w->tok_table;
@@ -356,11 +345,17 @@ int fast_step_enqueue(const ma_decoder_weights* w, SeqState s, int tmax, int max
       a.embed = (L == 0);
       if (L > 0) { a.hres_in = ws->hresB; a.y16_in = ws->y16; a.gamma = w->ln2g[L - 1]; a.beta = w->ln2b[L - 1]; }
       a.hres_out = ws->hresA;
-      a.out16 = ws->q; a.kc = kc; a.vc = vc;
+      a.out16 = ws->qkv;
       if (launch_fast<HID, MODE_QKV>(a, grid, pdl, st)) return 1;
     }
-    if (launch_attention_ex(ws->q, HID, kc, vc, T, NHEAD, 1, nullptr, &ws->nkeys, max_keys, 1, 0.125f, ws->attn16, HID,
-                            ws->attn_scratch, 1, pdl, st)) return 1;
+    if (!no_stream_attn()) {
+      if (launch_attention_decode(ws->qkv, QKV, kc, vc, T, &ws->nkeys, max_keys, 1, 0.125f, ws->attn16, HID,
+                                  ws->attn_scratch, pdl, st)) return 1;
+    } else {
+      if (launch_kv_append(ws->qkv, 1, 1, &ws->nkeys, kc, vc, T, st)) return 1;
+      if (launch_attention_ex(ws->qkv, QKV, kc, vc, T, NHEAD, 1, nullptr, &ws->nkeys, max_keys, 1, 0.125f, ws->attn16,
+                              HID, ws->attn_scratch, 1, pdl, st)) return 1;
+    }
     {  // out_proj
       FastArgs a = base;
       a.W = (const __half*)w->wo[L]; a.bias = (const __half*)w->bo[L]; a.N = HID; a.rows_per_cta = rpc(HID);

@@ -63,6 +63,8 @@ int launch_attention_decode(const __half* qkv, int ldq, __half* K, __half* V, lo
 int launch_attention(const __half* q, int ldq, const __half* K, const __half* V, long T, int H, int rows_per_slot,
                      const int* slots, const int* nkeys, int max_keys, int M, float scale, __half* out, int ldo,
                      void* scratch, cudaStream_t st);
+// api.cu: MA_B200_NO_STREAM_ATTN=1 -- decode attention on kv_append_kernel + attention_kernel instead
+bool no_stream_attn();
 
 // elementwise.cu
 int launch_layernorm(const float* x, const __half* res16, const float* gamma, const float* beta, float eps, int M,

@@ -42,7 +42,9 @@ def card():
 
 
 def op_of(name):
-    if "attention_kernel" in name:
+    # attention_stream_kernel: the decode steps; attention_kernel: the prefill, and the decode steps under
+    # MA_B200_NO_STREAM_ATTN=1 (whose kv_append_kernel is not matched: its time falls into the attention increment)
+    if "attention_stream_kernel" in name or "attention_kernel" in name:
         return "attention"
     if "fast_gemv_kernel" in name:
         mode = name.split("fast_gemv_kernel<", 1)[1].split(">", 1)[0].split(",")[1].strip()
