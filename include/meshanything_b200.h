@@ -427,6 +427,26 @@ int ma_remove_plane(const float* xyz, int n, int h, float t, unsigned long long 
  * compaction (NULL: off). */
 void ma_remove_plane_set_events(void* const* events);
 
+/* ---- splitting a point cloud into objects (`--split_objects`; csrc/objects.cu) ------------------------------------
+ * xyz fp32 [n][3], finite, already in the output frame -> what DESIGN.md section 1.7 defines: points i and j are
+ * neighbours iff ((dx dx + dy dy) + dz dz) <= e2 = fp32(e e) in fp32 without contraction; the clusters are the connected
+ * components of that graph, each labelled by its lowest point index, ordered by size (descending, the lowest label
+ * first on ties); the objects are the clusters of at least min_points points, in that order.
+ * Device outputs: labels_out int32 [n] (the label of every point), indices_out int64 [n] (the first stats_out[2]
+ * entries: the points of object 0 ascending, then object 1, ...), offsets_out int64 [n / min_points + 1] (the first
+ * objects + 1 entries: where each object starts in indices_out, then its end; the rest repeat the end), stats_out int64
+ * [6] = (clusters, objects, points in objects, dropped clusters, points in dropped clusters, largest dropped cluster).
+ * 1 <= n <= 2^24, 1 <= min_points <= n, 0 < e <= 1 with e e > 0 in fp32.  ws: ma_split_objects_workspace_bytes(n,
+ * min_points) bytes (no device needed; 0 for shapes out of range).  No host synchronisation and no floating-point
+ * atomics: two calls give identical bits. */
+size_t ma_split_objects_workspace_bytes(int n, int min_points);
+int ma_split_objects(const float* xyz, int n, float e, int min_points, int32_t* labels_out, int64_t* indices_out,
+                     int64_t* offsets_out, int64_t* stats_out, void* ws, void* stream);
+/* Measurement hook (tools/bench_objects.py): events = 4 cudaEvent_t recorded on the stream of every following call at
+ * its start and after the grid (box, cell keys, sort, occupied cells), the connectivity (cells, pairs, labels and
+ * sizes) and the order and selection (NULL: off). */
+void ma_split_objects_set_events(void* const* events);
+
 /* number of kernels launched by the library since load (bench.py's gpu_launches) */
 unsigned long long ma_launch_count(void);
 

@@ -5,6 +5,8 @@
     python main.py --input_type pc --input_path scan.npy --remove_outliers   # drop stray points / floaters first
     python main.py --input_type pc --input_path scan.npy --subsample fps     # even coverage of uneven scan density
     python main.py --input_type pc --input_path scan.npy --remove_plane      # drop the table / floor under the object
+    python main.py --input_type pc --input_path scan.npy --remove_plane --split_objects --output_frame input
+                                                   # one mesh per object on the table, each where it stands in the scan
     torchrun --nproc-per-node 8 main.py --input_type pc_normal --input_dir pcs --batchsize_per_gpu 64
 
 Differences forced by the environment: no accelerate / hf_hub (there is no network) -- one process per
@@ -58,6 +60,22 @@ def _remove_plane(xyz, path, plane, n_points=4096):
     return idx.cpu().numpy()
 
 
+def _split_objects(xyz, path, objects, n_points=4096):
+    """`--split_objects`: the point indices of every object of xyz [N, 3] that DESIGN.md section 1.7 defines (on the
+    GPU, meshanything_b200.objects), objects in order, each ascending; one line per input with the clusters, the
+    objects' sizes and the dropped points, e in the input's units."""
+    from meshanything_b200.objects import split_objects
+    idx, offsets, st = split_objects(xyz, min_points=n_points, **objects)
+    print(f"{_uid_of(path)}: {st.clusters} clusters at e = {st.distance:.4g} in input units; {st.objects} objects of "
+          f"{', '.join(str(s) for s in st.sizes) or 'no'} points; dropped {st.dropped_points} points in "
+          f"{st.dropped_clusters} smaller clusters (the largest {st.largest_dropped})")
+    if st.objects == 0:
+        raise ValueError(f"{path}: no cluster of {n_points} points at e = {st.distance:.4g} ({st.clusters} clusters, "
+                         f"the largest of {st.largest_dropped} points), fewer than the {n_points} the model takes")
+    idx, offsets = idx.cpu().numpy(), offsets.cpu().numpy()
+    return [idx[offsets[k]:offsets[k + 1]] for k in range(st.objects)]
+
+
 def _farthest_points(xyz, path, n_points=4096):
     """`--subsample fps`: the picks of farthest-point sampling (DESIGN.md section 1.4, on the GPU,
     meshanything_b200.subsample) from a start drawn from the global numpy RNG, so --seed still selects the subset; one
@@ -70,32 +88,43 @@ def _farthest_points(xyz, path, n_points=4096):
     return idx.cpu().numpy()
 
 
-def _subsample_points(path, n_points=4096, outliers=None, subsample='random', plane=None):
+def _subsample_points(path, n_points=4096, outliers=None, subsample='random', plane=None, objects=None):
     """`--input_type pc_normal`: an .npy of >= 4096 (xyz, normal) rows; a random 4096-subset without replacement
     (global numpy RNG, seeded by --seed as the reference does through accelerate.set_seed), or with
     subsample='fps' the farthest-point subset of the xyz columns.  With `outliers` (the keyword arguments of
     meshanything_b200.outliers.remove_outliers) the rows are first cleaned by their xyz; with `plane` (the keyword
-    arguments of meshanything_b200.plane.remove_plane) the support plane goes before that."""
+    arguments of meshanything_b200.plane.remove_plane) the support plane goes before that.  With `objects` ({'distance':
+    e}) the cleaned cloud is split into objects and a list of one subset per object is returned, drawn in object
+    order."""
     cloud = np.load(path)
     if plane is not None:
         cloud = cloud[_remove_plane(cloud[:, :3], path, plane, n_points)]
     if outliers is not None:
         cloud = cloud[_remove_outliers(cloud[:, :3], path, outliers, n_points)]
     assert cloud.shape[0] >= n_points, "input pc_normal should have at least 4096 points"
+    if objects is not None:
+        return [_subset(cloud[part], path, n_points, subsample)
+                for part in _split_objects(cloud[:, :3], path, objects, n_points)]
+    return _subset(cloud, path, n_points, subsample)
+
+
+def _subset(cloud, path, n_points, subsample):
+    """The 4096 rows of a cloud the model sees: random without replacement (global numpy RNG) or farthest points."""
     if subsample == 'fps':
         return cloud[_farthest_points(cloud[:, :3], path, n_points)]
     keep = np.random.choice(cloud.shape[0], n_points, replace=False)
     return cloud[keep]
 
 
-def _points_with_normals(path, n_points=4096, k=16, outliers=None, subsample='random', plane=None):
+def _points_with_normals(path, n_points=4096, k=16, outliers=None, subsample='random', plane=None, objects=None):
     """`--input_type pc`: a bare cloud (.npy (N, 3) or vertex-only .ply) of >= 4096 points.  Normals are estimated on
     the GPU from all N points (meshanything_b200.normals), then the same 4096-subset as `pc_normal` is drawn: the
     xyz-only copy of a file selects the points the file with normals selects under the same seed.  With `outliers`
     the cloud is cleaned first, and normals and subset come from the kept points; `plane` removes the support plane
-    before that."""
+    before that.  With `objects` the cleaned cloud is split into objects first, and every object gets its own normals
+    (estimated on its points alone, so that their orientation is rooted at its own farthest point) and subset, in
+    object order: a list of one cloud per object is returned."""
     from mesh_to_pc import load_points
-    from meshanything_b200.normals import estimate_normals
     xyz = load_points(path)
     if not np.issubdtype(xyz.dtype, np.floating):
         xyz = xyz.astype(np.float64)
@@ -104,6 +133,15 @@ def _points_with_normals(path, n_points=4096, k=16, outliers=None, subsample='ra
         xyz = xyz[_remove_plane(xyz, path, plane, n_points)]
     if outliers is not None:
         xyz = xyz[_remove_outliers(xyz, path, outliers, n_points)]
+    if objects is not None:
+        return [_with_normals(xyz[part], path, n_points, k, subsample)
+                for part in _split_objects(xyz, path, objects, n_points)]
+    return _with_normals(xyz, path, n_points, k, subsample)
+
+
+def _with_normals(xyz, path, n_points, k, subsample):
+    """Normals of every point of xyz on the GPU, then the subset: (4096, 6) rows."""
+    from meshanything_b200.normals import estimate_normals
     normals = estimate_normals(xyz, k).cpu().numpy()
     if subsample == 'fps':
         keep = _farthest_points(xyz, path, n_points)
@@ -120,9 +158,12 @@ _NO_MESH_OUTLIERS = ("--remove_outliers applies to point-cloud input (--input_ty
                      "mesh are sampled from its surface and have no outliers")
 _NO_MESH_FPS = ("--subsample fps applies to point-cloud input (--input_type pc or pc_normal): the points of a mesh are "
                 "already sampled uniformly by area")
+_NO_MESH_OBJECTS = ("--split_objects applies to point-cloud input (--input_type pc or pc_normal): splitting a mesh into "
+                    "its connected parts is not supported")
 _NO_MESH_PLANE = ("--remove_plane applies to point-cloud input (--input_type pc or pc_normal): the points of a mesh are "
                   "sampled from its own surface, which has no scanned support under it")
 SUBSAMPLERS = ('random', 'fps')
+OUTPUT_FRAMES = ('model', 'input')
 
 
 def _check_subsample(input_type, subsample):
@@ -138,25 +179,36 @@ class Dataset:
     clouds only): None, or the keyword arguments of meshanything_b200.outliers.remove_outliers, to clean every cloud
     before normals and subset.  `subsample` (point clouds only): 'random' (the reference's np.random.choice) or 'fps'
     (farthest-point sampling on the GPU, DESIGN.md section 1.4).  `plane` (point clouds only): None, or the keyword
-    arguments of meshanything_b200.plane.remove_plane, to remove the support plane (a table, the floor) first."""
+    arguments of meshanything_b200.plane.remove_plane, to remove the support plane (a table, the floor) first.
+    `objects` (point clouds only): None, or {'distance': e}, to split every cloud after plane and outlier removal into
+    objects (DESIGN.md section 1.7), each its own item with uid `{uid}_obj{k}`.  Items also carry 'frame', the
+    metrics.shape_frame of the rows before normalisation, which metrics.to_input_frame applies to put a mesh back in
+    the input's coordinates."""
 
-    def __init__(self, input_type, input_list, mc=False, outliers=None, subsample='random', plane=None):
+    def __init__(self, input_type, input_list, mc=False, outliers=None, subsample='random', plane=None, objects=None):
         if outliers is not None and input_type not in ('pc', 'pc_normal'):
             raise ValueError(_NO_MESH_OUTLIERS)
         if plane is not None and input_type not in ('pc', 'pc_normal'):
             raise ValueError(_NO_MESH_PLANE)
+        if objects is not None and input_type not in ('pc', 'pc_normal'):
+            raise ValueError(_NO_MESH_OBJECTS)
         _check_subsample(input_type, subsample)
+        kw = dict(outliers=outliers, subsample=subsample, plane=plane, objects=objects)
         if input_type == 'pc_normal':
-            clouds = [_subsample_points(p, outliers=outliers, subsample=subsample, plane=plane) for p in input_list]
+            clouds = [_subsample_points(p, **kw) for p in input_list]
         elif input_type == 'pc':
-            clouds = [_points_with_normals(p, outliers=outliers, subsample=subsample, plane=plane) for p in input_list]
+            clouds = [_points_with_normals(p, **kw) for p in input_list]
         elif input_type == 'mesh':
             if mc:
                 print("First Marching Cubes and then sample point cloud, need several minutes...")
             clouds, _ = process_mesh_to_pc([load_mesh(p) for p in input_list], marching_cubes=mc)
         else:
             raise ValueError(f"unknown input_type {input_type!r}")
-        self.data = [{'pc_normal': c, 'uid': _uid_of(p)} for c, p in zip(clouds, input_list)]
+        if objects is None:
+            self.data = [{'pc_normal': c, 'uid': _uid_of(p)} for c, p in zip(clouds, input_list)]
+        else:
+            self.data = [{'pc_normal': c, 'uid': f"{_uid_of(p)}_obj{k}"}
+                         for cs, p in zip(clouds, input_list) for k, c in enumerate(cs)]
         print(f"dataset total data samples: {len(self.data)}")
 
     def __len__(self):
@@ -164,8 +216,10 @@ class Dataset:
 
     def __getitem__(self, idx):
         from meshanything_b200.inputs import normalize_pc_normal
+        from meshanything_b200.metrics import shape_frame
         entry = self.data[idx]
-        return {'pc_normal': normalize_pc_normal(entry['pc_normal']), 'uid': entry['uid']}
+        return {'pc_normal': normalize_pc_normal(entry['pc_normal']), 'uid': entry['uid'],
+                'frame': shape_frame(entry['pc_normal'][:, :3])}
 
 
 _FLAGS = [  # (flag, default, type) -- the reference's command line (main.py:60-89)
@@ -206,6 +260,13 @@ def get_args():
     parser.add_argument('--remove_plane', default=False, action="store_true")
     parser.add_argument('--plane_distance', default=0.01, type=float)
     parser.add_argument('--plane_iterations', default=1000, type=int)
+    # not in the reference: split every cloud into objects (connected components at --object_distance of the bounding
+    # box's longest side; DESIGN.md section 1.7; meshanything_b200.objects) and mesh each one on its own
+    parser.add_argument('--split_objects', default=False, action="store_true")
+    parser.add_argument('--object_distance', default=0.02, type=float)
+    # not in the reference: write meshes in the model's [-0.5, 0.5) frame (model, the reference's output) or back in
+    # the input's coordinates (input: c + L v with the bounding box centre c and longest side L of the shape's points)
+    parser.add_argument('--output_frame', default='model', choices=OUTPUT_FRAMES)
     return parser.parse_args()
 
 
@@ -222,6 +283,13 @@ def plane_options(args):
     if not getattr(args, 'remove_plane', False):
         return None
     return {'distance': getattr(args, 'plane_distance', 0.01), 'iterations': getattr(args, 'plane_iterations', 1000)}
+
+
+def object_options(args):
+    """The `objects` argument of Dataset from the command line: None without --split_objects."""
+    if not getattr(args, 'split_objects', False):
+        return None
+    return {'distance': getattr(args, 'object_distance', 0.02)}
 
 
 def check_args(args):
@@ -251,6 +319,15 @@ def check_args(args):
                              f"{distance}")
         if not 1 <= iterations <= 65536:
             raise ValueError(f"--plane_iterations must be in 1..65536, got {iterations}")
+    if getattr(args, 'split_objects', False):
+        if args.input_type == 'mesh':
+            raise ValueError(_NO_MESH_OBJECTS)
+        distance = getattr(args, 'object_distance', 0.02)
+        if not (np.isfinite(distance) and 0 < distance <= 1 and np.float32(distance) * np.float32(distance) > 0):
+            raise ValueError(f"--object_distance must be in (0, 1] (a share of the bounding box's longest side, with a "
+                             f"square above 0 in fp32), got {distance}")
+    if getattr(args, 'output_frame', 'model') not in OUTPUT_FRAMES:
+        raise ValueError(f"--output_frame must be one of {', '.join(OUTPUT_FRAMES)}, got {args.output_frame!r}")
 
 
 def load_model(args, device=None):
@@ -375,7 +452,7 @@ if __name__ == "__main__":
     np.random.seed(args.seed)
     torch.manual_seed(args.seed)
     dataset = Dataset(args.input_type, input_list, args.mc, outliers=outlier_options(args), subsample=args.subsample,
-                      plane=plane_options(args))
+                      plane=plane_options(args), objects=object_options(args))
 
     bs = args.batchsize_per_gpu
     batches = [list(range(i, min(i + bs, len(dataset)))) for i in range(0, len(dataset), bs)]
@@ -384,6 +461,9 @@ if __name__ == "__main__":
 
     def save(item, recon_mesh):
         recon_mesh = recon_mesh[~torch.isnan(recon_mesh[:, 0, 0])]
+        if args.output_frame == 'input':
+            from meshanything_b200.metrics import to_input_frame
+            recon_mesh = to_input_frame(recon_mesh, item['frame'])
         save_path = os.path.join(checkpoint_dir, f'{item["uid"]}_gen.obj')
         export_obj(save_path, recon_mesh.cpu().numpy())
         print(f"{save_path} Over!!")

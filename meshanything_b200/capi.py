@@ -54,6 +54,7 @@ EXPORTS = [
     "ma_farthest_point_sample_workspace_bytes", "ma_farthest_point_sample", "ma_farthest_point_sample_set_path",
     "ma_farthest_point_sample_last_path",
     "ma_remove_plane_workspace_bytes", "ma_remove_plane", "ma_remove_plane_set_events",
+    "ma_split_objects_workspace_bytes", "ma_split_objects", "ma_split_objects_set_events",
     "ma_fourier_embed_f16", "ma_scatter_heads_f16", "ma_residual_add", "ma_convert_rows", "ma_add_table",
     "ma_gather_codes", "ma_coords",
 ]
@@ -156,6 +157,11 @@ def lib():
                                   _vp]
     L.ma_remove_plane_set_events.argtypes = [_vp]
     L.ma_remove_plane_set_events.restype = None
+    L.ma_split_objects_workspace_bytes.argtypes = [C.c_int, C.c_int]
+    L.ma_split_objects_workspace_bytes.restype = C.c_size_t
+    L.ma_split_objects.argtypes = [_vp, C.c_int, C.c_float, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp]
+    L.ma_split_objects_set_events.argtypes = [_vp]
+    L.ma_split_objects_set_events.restype = None
     L.ma_fourier_embed_f16.argtypes = [_vp, C.c_long, _vp, _vp]
     L.ma_scatter_heads_f16.argtypes = [_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_long, _vp, C.c_long, _vp]
     L.ma_residual_add.argtypes = [_vp, _vp, _vp, C.c_long, _vp]
@@ -577,6 +583,59 @@ def remove_plane(points: torch.Tensor, distance: float = 0.01, iterations: int =
         st = stats.cpu().numpy()
     out = (idx[:int(st[11])], keep.bool(), st)
     return (*out, counts, planes) if want_terms else out
+
+
+def split_objects(points: torch.Tensor, distance: float = 0.02, min_points: int = 4096):
+    """Splitting a cloud into objects (ma_split_objects; objects.split_objects adds the frame map).
+
+    points fp32 [N, 3], contiguous, on a CUDA device, finite, already in the output frame; 1 <= N <= 2^24; distance
+    the neighbour distance e in the frame, 0 < e <= 1 (rounded to fp32; fp32(e e) must stay > 0); 1 <= min_points <= N.
+    Returns (labels int32 [N], object indices int64 [points in objects], offsets int64 [objects + 1], stats int64 [6]
+    on the host: clusters, objects, points in objects, dropped clusters, points in dropped clusters, largest dropped
+    cluster).  Every bad input raises ValueError before anything is launched.  Reads the stats back (synchronises)."""
+    if not isinstance(points, torch.Tensor):
+        raise ValueError(f"split_objects: points must be a torch tensor, got {type(points).__name__}")
+    if points.dim() != 2 or points.shape[1] != 3:
+        raise ValueError(f"split_objects: points [N, 3], got {tuple(points.shape)}")
+    if points.dtype != torch.float32:
+        raise ValueError(f"split_objects: points must be float32, got {points.dtype}")
+    if not points.is_contiguous():
+        raise ValueError("split_objects: points must be contiguous")
+    if not points.is_cuda:
+        raise ValueError("split_objects: points must live on a CUDA device (no CPU fallback)")
+    n = points.shape[0]
+    if not 1 <= n <= 1 << 24:
+        raise ValueError(f"split_objects: 1 <= N <= 2^24, got N = {n}")
+    if isinstance(min_points, bool):
+        raise ValueError("split_objects: min_points must be an integer")
+    try:
+        min_points = operator.index(min_points)
+    except TypeError:
+        raise ValueError(f"split_objects: min_points must be an integer, got {min_points!r}") from None
+    if not 1 <= min_points <= n:
+        raise ValueError(f"split_objects: 1 <= min_points <= N = {n}, got {min_points}")
+    if isinstance(distance, bool):
+        raise ValueError("split_objects: distance must be a real number")
+    try:
+        distance = float(distance)
+    except (TypeError, ValueError):
+        raise ValueError(f"split_objects: distance must be a real number, got {distance!r}") from None
+    e32 = C.c_float(distance).value
+    if not (math.isfinite(distance) and 0 < distance <= 1 and 0 < e32 <= 1 and C.c_float(e32 * e32).value > 0):
+        raise ValueError(f"split_objects: 0 < distance <= 1 (and its fp32 square > 0), got {distance}")
+    if not bool(torch.isfinite(points).all()):
+        raise ValueError("split_objects: non-finite coordinates")
+    dev = points.device
+    ws = torch.empty(lib().ma_split_objects_workspace_bytes(n, min_points), dtype=torch.uint8, device=dev)
+    labels = torch.empty((n,), dtype=torch.int32, device=dev)
+    idx = torch.empty((n,), dtype=torch.int64, device=dev)
+    offsets = torch.empty((n // min_points + 1,), dtype=torch.int64, device=dev)
+    stats = torch.empty((6,), dtype=torch.int64, device=dev)
+    with torch.cuda.device(dev):
+        check(lib().ma_split_objects(ptr(points), n, C.c_float(e32), min_points, ptr(labels), ptr(idx), ptr(offsets),
+                                     ptr(stats), ptr(ws), stream_ptr()), "ma_split_objects")
+        st = stats.cpu().numpy()
+    return labels, idx[:int(st[2])], offsets[:int(st[1]) + 1], st
 
 
 def tensor_core_linear_counts():

@@ -30,6 +30,23 @@ def to_output_frame(pc_normal: torch.Tensor) -> torch.Tensor:
     return torch.cat([(xyz - centre) / side, pc[..., 3:]], dim=-1)
 
 
+def shape_frame(xyz) -> tuple:
+    """The map to_output_frame applies to rows [P, 3] (any float dtype), in float64: (centre [3], longest side), the
+    bounding box's centre and longest side, 0 counting as 1."""
+    p = torch.as_tensor(xyz).to(torch.float64)
+    lo, hi = p.amin(dim=0), p.amax(dim=0)
+    side = float((hi - lo).max())
+    return (lo + hi) / 2, side if side > 0 else 1.0
+
+
+def to_input_frame(faces: torch.Tensor, frame: tuple) -> torch.Tensor:
+    """The inverse of to_output_frame in float64: every coordinate v of `faces` (any shape [..., 3]) becomes
+    centre + side v, with frame = shape_frame of the cloud the faces were generated from."""
+    centre, side = frame
+    v = torch.as_tensor(faces).to(torch.float64)
+    return centre.to(v.device) + side * v
+
+
 def score(meshes: torch.Tensor, pc_normal: torch.Tensor) -> dict:
     """Score candidate meshes against the clouds they were generated from.
 
