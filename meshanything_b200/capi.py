@@ -198,6 +198,56 @@ def _need_cuda(*ts):
             raise RuntimeError("meshanything_b200: tensors must live on a CUDA device (no CPU fallback)")
 
 
+def _check_points(what: str, points, n_min: int) -> int:
+    """N of a cloud handed to a point-cloud entry point: ValueError unless `points` is a contiguous fp32 [N, 3] CUDA
+    tensor of finite coordinates with n_min <= N <= 2^24."""
+    if not isinstance(points, torch.Tensor):
+        raise ValueError(f"{what}: points must be a torch tensor, got {type(points).__name__}")
+    if points.dim() != 2 or points.shape[1] != 3:
+        raise ValueError(f"{what}: points [N, 3], got {tuple(points.shape)}")
+    if points.dtype != torch.float32:
+        raise ValueError(f"{what}: points must be float32, got {points.dtype}")
+    if not points.is_contiguous():
+        raise ValueError(f"{what}: points must be contiguous")
+    if not points.is_cuda:
+        raise ValueError(f"{what}: points must live on a CUDA device (no CPU fallback)")
+    n = points.shape[0]
+    if not n_min <= n <= 1 << 24:
+        raise ValueError(f"{what}: {n_min} <= N <= 2^24, got N = {n}")
+    if not bool(torch.isfinite(points).all()):
+        raise ValueError(f"{what}: non-finite coordinates")
+    return n
+
+
+def _check_int(what: str, name: str, value, lo: int, hi: int) -> int:
+    """`value` as an int in [lo, hi]; ValueError otherwise, and for bool, which operator.index would accept."""
+    if isinstance(value, bool):
+        raise ValueError(f"{what}: {name} must be an integer, got {value!r}")
+    try:
+        value = operator.index(value)
+    except TypeError:
+        raise ValueError(f"{what}: {name} must be an integer, got {value!r}") from None
+    if not lo <= value <= hi:
+        raise ValueError(f"{what}: {lo} <= {name} <= {hi}, got {value}")
+    return value
+
+
+def _check_share(what: str, name: str, value, square: bool = False) -> float:
+    """`value`, a share of the frame's side, rounded to fp32: ValueError unless it is a finite real number in (0, 1]
+    that stays above 0 in fp32 and, with `square`, whose fp32 square stays above 0 too."""
+    if isinstance(value, bool):
+        raise ValueError(f"{what}: {name} must be a real number")
+    try:
+        value = float(value)
+    except (TypeError, ValueError):
+        raise ValueError(f"{what}: {name} must be a real number, got {value!r}") from None
+    v32 = C.c_float(value).value
+    if not (math.isfinite(value) and 0 < value <= 1 and 0 < v32 <= 1 and (not square or C.c_float(v32 * v32).value > 0)):
+        rule = "its fp32 square > 0" if square else "> 0 in fp32"
+        raise ValueError(f"{what}: 0 < {name} <= 1 (and {rule}), got {value}")
+    return v32
+
+
 # ---------------------------------------------------------------- canonical building blocks
 
 def linear_f16(w: torch.Tensor, bias: Optional[torch.Tensor], x: torch.Tensor, epilogue: int = EPI_NONE,
@@ -421,25 +471,19 @@ def mesh_score(meshes: torch.Tensor, clouds: torch.Tensor, want_terms: bool = Fa
 def estimate_normals(points: torch.Tensor, k: int = 16, want_terms: bool = False):
     """Oriented unit normals of a bare cloud (ma_estimate_normals; normals.estimate_normals adds the frame map).
 
-    points fp32 [N, 3], finite, already in the output frame; 1 <= k <= 64, k < N <= 2^24.  Returns normals fp32 [N, 3];
-    with want_terms (normals, kNN int32 [N, k] in rank order, unoriented normals fp32 [N, 3])."""
-    _need_cuda(points)
-    p = points.to(torch.float32).contiguous()
-    if p.dim() != 2 or p.shape[1] != 3:
-        raise ValueError("estimate_normals: points [N, 3]")
-    n = p.shape[0]
-    if not 1 <= k <= 64:
-        raise ValueError(f"estimate_normals: 1 <= k <= 64, got k = {k}")
-    if not k < n <= 1 << 24:
-        raise ValueError(f"estimate_normals: k < N <= 2^24, got N = {n}, k = {k}")
-    if not bool(torch.isfinite(p).all()):
-        raise ValueError("estimate_normals: non-finite coordinates")
-    ws = torch.empty(lib().ma_estimate_normals_workspace_bytes(n, k), dtype=torch.uint8, device=p.device)
-    out = torch.empty((n, 3), dtype=torch.float32, device=p.device)
-    knn = torch.empty((n, k), dtype=torch.int32, device=p.device) if want_terms else None
-    uno = torch.empty((n, 3), dtype=torch.float32, device=p.device) if want_terms else None
-    check(lib().ma_estimate_normals(ptr(p), n, k, ptr(out), ptr(knn), ptr(uno), ptr(ws), stream_ptr()),
-          "ma_estimate_normals")
+    points fp32 [N, 3], contiguous, on a CUDA device, finite, already in the output frame; 1 <= k <= 64,
+    k < N <= 2^24.  Returns normals fp32 [N, 3]; with want_terms (normals, kNN int32 [N, k] in rank order, unoriented
+    normals fp32 [N, 3]).  Every bad input raises ValueError before anything is launched."""
+    k = _check_int("estimate_normals", "k", k, 1, 64)
+    n = _check_points("estimate_normals", points, k + 1)
+    dev = points.device
+    ws = torch.empty(lib().ma_estimate_normals_workspace_bytes(n, k), dtype=torch.uint8, device=dev)
+    out = torch.empty((n, 3), dtype=torch.float32, device=dev)
+    knn = torch.empty((n, k), dtype=torch.int32, device=dev) if want_terms else None
+    uno = torch.empty((n, 3), dtype=torch.float32, device=dev) if want_terms else None
+    with torch.cuda.device(dev):
+        check(lib().ma_estimate_normals(ptr(points), n, k, ptr(out), ptr(knn), ptr(uno), ptr(ws), stream_ptr()),
+              "ma_estimate_normals")
     return (out, knn, uno) if want_terms else out
 
 
@@ -447,26 +491,18 @@ def remove_outliers(points: torch.Tensor, k: int = 16, std_ratio: float = 2.0, m
                     want_terms: bool = False):
     """Outlier removal of a cloud (ma_remove_outliers; outliers.remove_outliers adds the frame map).
 
-    points fp32 [N, 3], finite, already in the output frame; 1 <= k <= 64, k < N <= 2^24.  Returns (kept indices int64
-    [n_kept] ascending, keep mask bool [N], stats fp64 [8] on the host: mu, sigma, threshold, statistical inliers,
-    components, components dropped, kept points, connectivity rounds); with want_terms also (mean neighbour distance
-    fp64 [N], kNN int32 [N, k] in rank order).  Reads the stats back (synchronises)."""
-    _need_cuda(points)
-    p = points.to(torch.float32).contiguous()
-    if p.dim() != 2 or p.shape[1] != 3:
-        raise ValueError("remove_outliers: points [N, 3]")
-    n = p.shape[0]
-    if not 1 <= k <= 64:
-        raise ValueError(f"remove_outliers: 1 <= k <= 64, got k = {k}")
-    if not k < n <= 1 << 24:
-        raise ValueError(f"remove_outliers: k < N <= 2^24, got N = {n}, k = {k}")
+    points fp32 [N, 3], contiguous, on a CUDA device, finite, already in the output frame; 1 <= k <= 64,
+    k < N <= 2^24.  Returns (kept indices int64 [n_kept] ascending, keep mask bool [N], stats fp64 [8] on the host: mu,
+    sigma, threshold, statistical inliers, components, components dropped, kept points, connectivity rounds); with
+    want_terms also (mean neighbour distance fp64 [N], kNN int32 [N, k] in rank order).  Every bad input raises
+    ValueError before anything is launched.  Reads the stats back (synchronises)."""
+    k = _check_int("remove_outliers", "k", k, 1, 64)
+    n = _check_points("remove_outliers", points, k + 1)
     if not math.isfinite(std_ratio):
         raise ValueError(f"remove_outliers: std_ratio must be finite, got {std_ratio}")
     if not (math.isfinite(min_component) and min_component >= 0):
         raise ValueError(f"remove_outliers: min_component must be finite and >= 0, got {min_component}")
-    if not bool(torch.isfinite(p).all()):
-        raise ValueError("remove_outliers: non-finite coordinates")
-    dev = p.device
+    dev = points.device
     ws = torch.empty(lib().ma_remove_outliers_workspace_bytes(n, k), dtype=torch.uint8, device=dev)
     keep = torch.empty((n,), dtype=torch.uint8, device=dev)
     idx = torch.empty((n,), dtype=torch.int64, device=dev)
@@ -474,10 +510,11 @@ def remove_outliers(points: torch.Tensor, k: int = 16, std_ratio: float = 2.0, m
     stats = torch.empty((8,), dtype=torch.float64, device=dev)
     mean = torch.empty((n,), dtype=torch.float64, device=dev) if want_terms else None
     knn = torch.empty((n, k), dtype=torch.int32, device=dev) if want_terms else None
-    check(lib().ma_remove_outliers(ptr(p), n, k, C.c_double(std_ratio), C.c_double(min_component), ptr(keep), ptr(idx),
-                                   ptr(n_kept), ptr(mean), ptr(knn), ptr(stats), ptr(ws), stream_ptr()),
-          "ma_remove_outliers")
-    st = stats.cpu().numpy()
+    with torch.cuda.device(dev):
+        check(lib().ma_remove_outliers(ptr(points), n, k, C.c_double(std_ratio), C.c_double(min_component), ptr(keep),
+                                       ptr(idx), ptr(n_kept), ptr(mean), ptr(knn), ptr(stats), ptr(ws), stream_ptr()),
+              "ma_remove_outliers")
+        st = stats.cpu().numpy()
     out = (idx[:int(st[6])], keep.bool(), st)
     return (*out, mean, knn) if want_terms else out
 
@@ -489,29 +526,9 @@ def farthest_point_sample(points: torch.Tensor, m: int, start: int = 0):
     points fp32 [N, 3], contiguous, on a CUDA device, finite, already in the output frame; 1 <= m <= N <= 2^24,
     0 <= start < N.  Returns (picks int64 [m] in pick order, r2 fp32 [m]: r2[t] the squared covering radius of the first
     t + 1 picks), both on the device.  Every bad input raises ValueError before anything is launched."""
-    if not isinstance(points, torch.Tensor):
-        raise ValueError(f"farthest_point_sample: points must be a torch tensor, got {type(points).__name__}")
-    if points.dim() != 2 or points.shape[1] != 3:
-        raise ValueError(f"farthest_point_sample: points [N, 3], got {tuple(points.shape)}")
-    if points.dtype != torch.float32:
-        raise ValueError(f"farthest_point_sample: points must be float32, got {points.dtype}")
-    if not points.is_contiguous():
-        raise ValueError("farthest_point_sample: points must be contiguous")
-    if not points.is_cuda:
-        raise ValueError("farthest_point_sample: points must live on a CUDA device (no CPU fallback)")
-    if isinstance(m, bool) or isinstance(start, bool):
-        raise ValueError("farthest_point_sample: m and start must be integers")
-    try:
-        m, start = operator.index(m), operator.index(start)
-    except TypeError:
-        raise ValueError(f"farthest_point_sample: m and start must be integers, got {m!r}, {start!r}") from None
-    n = points.shape[0]
-    if not 1 <= m <= n <= 1 << 24:
-        raise ValueError(f"farthest_point_sample: 1 <= m <= N <= 2^24, got N = {n}, m = {m}")
-    if not 0 <= start < n:
-        raise ValueError(f"farthest_point_sample: 0 <= start < N, got start = {start}, N = {n}")
-    if not bool(torch.isfinite(points).all()):
-        raise ValueError("farthest_point_sample: non-finite coordinates")
+    n = _check_points("farthest_point_sample", points, 1)
+    m = _check_int("farthest_point_sample", "m", m, 1, n)
+    start = _check_int("farthest_point_sample", "start", start, 0, n - 1)
     dev = points.device
     ws = torch.empty(lib().ma_farthest_point_sample_workspace_bytes(n, m), dtype=torch.uint8, device=dev)
     idx = torch.empty((m,), dtype=torch.int64, device=dev)
@@ -535,40 +552,10 @@ def remove_plane(points: torch.Tensor, distance: float = 0.01, iterations: int =
     stats fp64 [12] on the host: found, nx, ny, nz, d, winning hypothesis, its count, valid hypotheses, on, above,
     below, kept); with want_terms also (on-plane count int32 [H] and plane fp32 [H, 4] of every hypothesis).  Every bad
     input raises ValueError before anything is launched.  Reads the stats back (synchronises)."""
-    if not isinstance(points, torch.Tensor):
-        raise ValueError(f"remove_plane: points must be a torch tensor, got {type(points).__name__}")
-    if points.dim() != 2 or points.shape[1] != 3:
-        raise ValueError(f"remove_plane: points [N, 3], got {tuple(points.shape)}")
-    if points.dtype != torch.float32:
-        raise ValueError(f"remove_plane: points must be float32, got {points.dtype}")
-    if not points.is_contiguous():
-        raise ValueError("remove_plane: points must be contiguous")
-    if not points.is_cuda:
-        raise ValueError("remove_plane: points must live on a CUDA device (no CPU fallback)")
-    n = points.shape[0]
-    if not 3 <= n <= 1 << 24:
-        raise ValueError(f"remove_plane: 3 <= N <= 2^24, got N = {n}")
-    if isinstance(iterations, bool) or isinstance(seed, bool):
-        raise ValueError("remove_plane: iterations and seed must be integers")
-    try:
-        iterations, seed = operator.index(iterations), operator.index(seed)
-    except TypeError:
-        raise ValueError(f"remove_plane: iterations and seed must be integers, got {iterations!r}, {seed!r}") from None
-    if not 1 <= iterations <= PLANE_MAX_H:
-        raise ValueError(f"remove_plane: 1 <= iterations <= {PLANE_MAX_H}, got {iterations}")
-    if not 0 <= seed < 1 << 64:
-        raise ValueError(f"remove_plane: 0 <= seed < 2^64, got {seed}")
-    if isinstance(distance, bool):
-        raise ValueError("remove_plane: distance must be a real number")
-    try:
-        distance = float(distance)
-    except (TypeError, ValueError):
-        raise ValueError(f"remove_plane: distance must be a real number, got {distance!r}") from None
-    t32 = C.c_float(distance).value
-    if not (math.isfinite(distance) and 0 < distance <= 1 and 0 < t32 <= 1):
-        raise ValueError(f"remove_plane: 0 < distance <= 1 (and > 0 in fp32), got {distance}")
-    if not bool(torch.isfinite(points).all()):
-        raise ValueError("remove_plane: non-finite coordinates")
+    n = _check_points("remove_plane", points, 3)
+    iterations = _check_int("remove_plane", "iterations", iterations, 1, PLANE_MAX_H)
+    seed = _check_int("remove_plane", "seed", seed, 0, (1 << 64) - 1)
+    t32 = _check_share("remove_plane", "distance", distance)
     dev = points.device
     ws = torch.empty(lib().ma_remove_plane_workspace_bytes(n, iterations), dtype=torch.uint8, device=dev)
     keep = torch.empty((n,), dtype=torch.uint8, device=dev)
@@ -593,38 +580,9 @@ def split_objects(points: torch.Tensor, distance: float = 0.02, min_points: int 
     Returns (labels int32 [N], object indices int64 [points in objects], offsets int64 [objects + 1], stats int64 [6]
     on the host: clusters, objects, points in objects, dropped clusters, points in dropped clusters, largest dropped
     cluster).  Every bad input raises ValueError before anything is launched.  Reads the stats back (synchronises)."""
-    if not isinstance(points, torch.Tensor):
-        raise ValueError(f"split_objects: points must be a torch tensor, got {type(points).__name__}")
-    if points.dim() != 2 or points.shape[1] != 3:
-        raise ValueError(f"split_objects: points [N, 3], got {tuple(points.shape)}")
-    if points.dtype != torch.float32:
-        raise ValueError(f"split_objects: points must be float32, got {points.dtype}")
-    if not points.is_contiguous():
-        raise ValueError("split_objects: points must be contiguous")
-    if not points.is_cuda:
-        raise ValueError("split_objects: points must live on a CUDA device (no CPU fallback)")
-    n = points.shape[0]
-    if not 1 <= n <= 1 << 24:
-        raise ValueError(f"split_objects: 1 <= N <= 2^24, got N = {n}")
-    if isinstance(min_points, bool):
-        raise ValueError("split_objects: min_points must be an integer")
-    try:
-        min_points = operator.index(min_points)
-    except TypeError:
-        raise ValueError(f"split_objects: min_points must be an integer, got {min_points!r}") from None
-    if not 1 <= min_points <= n:
-        raise ValueError(f"split_objects: 1 <= min_points <= N = {n}, got {min_points}")
-    if isinstance(distance, bool):
-        raise ValueError("split_objects: distance must be a real number")
-    try:
-        distance = float(distance)
-    except (TypeError, ValueError):
-        raise ValueError(f"split_objects: distance must be a real number, got {distance!r}") from None
-    e32 = C.c_float(distance).value
-    if not (math.isfinite(distance) and 0 < distance <= 1 and 0 < e32 <= 1 and C.c_float(e32 * e32).value > 0):
-        raise ValueError(f"split_objects: 0 < distance <= 1 (and its fp32 square > 0), got {distance}")
-    if not bool(torch.isfinite(points).all()):
-        raise ValueError("split_objects: non-finite coordinates")
+    n = _check_points("split_objects", points, 1)
+    min_points = _check_int("split_objects", "min_points", min_points, 1, n)
+    e32 = _check_share("split_objects", "distance", distance, square=True)
     dev = points.device
     ws = torch.empty(lib().ma_split_objects_workspace_bytes(n, min_points), dtype=torch.uint8, device=dev)
     labels = torch.empty((n,), dtype=torch.int32, device=dev)

@@ -16,8 +16,11 @@
 
 #include <cstdint>
 
+#include <cub/device/device_scan.cuh>
+
 namespace ma {
 
+constexpr int kKnnBinThreads = 256;  // threads per CTA of knn_cell_kernel and knn_scatter_kernel
 constexpr int kKnnThreads = 64;   // kNN threads per CTA: k x 64 x 8 B of shared memory for the top-k lists
 constexpr int kKnnMaxK = 64;
 constexpr int kKnnMaxG = 256;
@@ -63,6 +66,28 @@ static __global__ void knn_scatter_kernel(const float* __restrict__ xyz, int n, 
   const uint32_t slot = start[c] + atomicSub(count + c, 1u) - 1u;
   const float* p = xyz + 3 * (size_t)i;
   sorted[slot] = make_float4(p[0], p[1], p[2], __int_as_float(i));
+}
+
+// bytes of CUB scratch that knn_bin needs for a grid of `cells` cells
+static inline size_t knn_bin_scan_bytes(size_t cells) {
+  size_t bytes = 0;
+  cub::DeviceScan::ExclusiveSum(nullptr, bytes, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)(cells + 1));
+  return bytes;
+}
+
+// The grid step on stream st: zero count[cells + 1], bin the points, scan the counts into start[], scatter the
+// points into sorted[] in cell order.  Stops at the first runtime error and returns it.  Launches are not counted.
+static inline cudaError_t knn_bin(const float* xyz, int n, const KnnGrid& g, uint32_t* cell, uint32_t* count,
+                                  uint32_t* start, float4* sorted, void* scan, size_t scan_bytes, cudaStream_t st) {
+  const size_t cells = (size_t)g.G * g.G * g.G;
+  const int nb = (n + kKnnBinThreads - 1) / kKnnBinThreads;
+  cudaError_t e = cudaMemsetAsync(count, 0, (cells + 1) * 4, st);
+  if (e != cudaSuccess) return e;
+  knn_cell_kernel<<<nb, kKnnBinThreads, 0, st>>>(xyz, n, g, cell, count);
+  e = cub::DeviceScan::ExclusiveSum(scan, scan_bytes, count, start, (int)(cells + 1), st);
+  if (e != cudaSuccess) return e;
+  knn_scatter_kernel<<<nb, kKnnBinThreads, 0, st>>>(xyz, n, cell, start, count, sorted);
+  return cudaSuccess;
 }
 
 // offers the candidates sorted[t0, t1) to the sorted top-k list top[e * kKnnThreads] (m entries so far)

@@ -13,8 +13,8 @@
 // Every fp32 step is an explicit round-to-nearest intrinsic and every fp64 sum runs in a fixed order with no atomics, so
 // a call is bit-deterministic and tests/mesh_score_oracle.py restates the per-point results bit for bit.
 #include "canon.cuh"
-#include "internal.h"
 #include "tri_dist.cuh"
+#include "workspace.h"
 
 namespace ma {
 
@@ -209,11 +209,26 @@ __global__ void mesh_score_reduce_kernel(const double* __restrict__ part_p, int 
   out_faces[sn] = (int32_t)cnt;
 }
 
-static size_t ms_align(size_t b) { return (b + 255) & ~(size_t)255; }
 static int ms_tiles_p(int P) { return (P + kMsThreads - 1) / kMsThreads; }
 static int ms_tiles_q(int F) { return (int)(((long long)F * kMsQuad + kMsThreads - 1) / kMsThreads); }
 static bool ms_shape_ok(int S, int N, int F, int P) {
   return S >= 1 && N >= 1 && F >= 1 && P >= 1 && (long long)S * N <= 65535 && F <= (1 << 26) && P <= (1 << 26);
+}
+
+// the per-tile partials of both directions
+struct MsBuffers {
+  double *part_p, *part_q;
+  size_t total;
+};
+
+static MsBuffers ms_buffers(int S, int N, int F, int P, void* ws) {
+  const size_t sn = (size_t)S * N;
+  Carver c(ws);
+  MsBuffers b;
+  b.part_p = c.take<double>(sn * ms_tiles_p(P) * 2);
+  b.part_q = c.take<double>(sn * ms_tiles_q(F) * 4);
+  b.total = c.total;
+  return b;
 }
 
 }  // namespace ma
@@ -224,8 +239,7 @@ extern "C" {
 
 size_t ma_mesh_score_workspace_bytes(int S, int N, int F, int P) {
   if (!ms_shape_ok(S, N, F, P)) return 0;
-  const size_t sn = (size_t)S * N;
-  return ms_align(sn * ms_tiles_p(P) * 2 * sizeof(double)) + ms_align(sn * ms_tiles_q(F) * 4 * sizeof(double));
+  return ms_buffers(S, N, F, P, nullptr).total;
 }
 
 int ma_mesh_score(const float* meshes, const float* clouds, int S, int N, int F, int P, double* out,
@@ -238,14 +252,12 @@ int ma_mesh_score(const float* meshes, const float* clouds, int S, int N, int F,
   }
   cudaStream_t st = (cudaStream_t)stream;
   const int sn = S * N, tiles_p = ms_tiles_p(P), tiles_q = ms_tiles_q(F);
-  double* part_p = reinterpret_cast<double*>(ws);
-  double* part_q = reinterpret_cast<double*>(reinterpret_cast<char*>(ws) +
-                                             ms_align((size_t)sn * tiles_p * 2 * sizeof(double)));
-  mesh_score_p2m_kernel<<<dim3(tiles_p, sn), kMsThreads, 0, st>>>(meshes, clouds, N, F, P, part_p, point_dist,
+  const MsBuffers b = ms_buffers(S, N, F, P, ws);
+  mesh_score_p2m_kernel<<<dim3(tiles_p, sn), kMsThreads, 0, st>>>(meshes, clouds, N, F, P, b.part_p, point_dist,
                                                                    point_face);
-  mesh_score_m2p_kernel<<<dim3(tiles_q, sn), kMsThreads, 0, st>>>(meshes, clouds, N, F, P, part_q, quad_dist,
+  mesh_score_m2p_kernel<<<dim3(tiles_q, sn), kMsThreads, 0, st>>>(meshes, clouds, N, F, P, b.part_q, quad_dist,
                                                                    quad_point);
-  mesh_score_reduce_kernel<<<(sn + 63) / 64, 64, 0, st>>>(part_p, tiles_p, part_q, tiles_q, sn, P, out, out_faces);
+  mesh_score_reduce_kernel<<<(sn + 63) / 64, 64, 0, st>>>(b.part_p, tiles_p, b.part_q, tiles_q, sn, P, out, out_faces);
   count_launch(3);
   return check_launch("ma_mesh_score") ? 0 : 1;
 }

@@ -19,12 +19,10 @@
 // Every fp32 step is an explicit round-to-nearest intrinsic, every fp64 step too (nvcc contracts fp64 as well), and
 // every choice is a minimum over unique keys, so a call is bit-deterministic and tests/normals_oracle.py restates the
 // neighbours, the unoriented and the oriented normals bit for bit.
-#include <cub/device/device_scan.cuh>
-
 #include "canon.cuh"
-#include "internal.h"
 #include "jacobi3.cuh"
 #include "knn_grid.cuh"
+#include "workspace.h"
 
 namespace ma {
 
@@ -214,51 +212,47 @@ __global__ void normals_apply_kernel(const float* __restrict__ xyz, const float*
 
 // ---------------------------------------------------------------- workspace
 
-static size_t nm_align(size_t b) { return (b + 255) & ~(size_t)255; }
 static bool nm_shape_ok(int n, int k) { return k >= 1 && k <= kKnnMaxK && n > k && n <= kNmMaxN; }
 
-static size_t nm_scan_bytes(size_t cells) {
-  size_t bytes = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, bytes, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)(cells + 1));
-  return bytes;
-}
-
-struct NmLayout {
-  size_t sorted, cell, count, start, scan, knn, uno, w, word, hook, best1, best2, hooks, total;
+struct NmBuffers {
+  float4* sorted;
+  uint32_t *cell, *count, *start;
+  void* scan;
+  size_t scan_bytes;
+  int32_t* knn;
+  float* uno;
+  uint32_t *w, *word, *hook;
+  unsigned long long* best1;
+  uint32_t* best2;
+  int* hooks;
+  size_t total;
 };
 
-static NmLayout nm_layout(int n, int k) {
+static NmBuffers nm_buffers(int n, int k, void* ws) {
   const int G = nm_grid(n, k).G;
   const size_t cells = (size_t)G * G * G, nk = (size_t)n * k;
-  NmLayout L;
-  size_t o = 0;
-  auto take = [&](size_t bytes) { const size_t at = o; o += nm_align(bytes); return at; };
-  L.sorted = take((size_t)n * sizeof(float4));
-  L.cell = take((size_t)n * 4);
-  L.count = take((cells + 1) * 4);
-  L.start = take((cells + 1) * 4);
-  L.scan = take(nm_scan_bytes(cells));
-  L.knn = take(nk * 4);
-  L.uno = take((size_t)n * 12);
-  L.w = take(nk * 4);
-  L.word = take((size_t)n * 4);
-  L.hook = take((size_t)n * 4);
-  L.best1 = take((size_t)n * 8);
-  L.best2 = take((size_t)n * 4);
-  L.hooks = take(4);
-  L.total = o;
-  return L;
+  Carver c(ws);
+  NmBuffers b;
+  b.sorted = c.take<float4>(n);
+  b.cell = c.take<uint32_t>(n);
+  b.count = c.take<uint32_t>(cells + 1);
+  b.start = c.take<uint32_t>(cells + 1);
+  b.scan_bytes = knn_bin_scan_bytes(cells);
+  b.scan = c.take<char>(b.scan_bytes);
+  b.knn = c.take<int32_t>(nk);
+  b.uno = c.take<float>(3 * (size_t)n);
+  b.w = c.take<uint32_t>(nk);
+  b.word = c.take<uint32_t>(n);
+  b.hook = c.take<uint32_t>(n);
+  b.best1 = c.take<unsigned long long>(n);
+  b.best2 = c.take<uint32_t>(n);
+  b.hooks = c.take<int>(1);
+  b.total = c.total;
+  return b;
 }
 
-static cudaEvent_t g_nm_events[5];
-static bool g_nm_timed = false;
+static StageEvents<5> nm_events;
 static int g_nm_rounds = 0;
-
-static void nm_mark(int at, cudaStream_t st) {
-  if (g_nm_timed) cudaEventRecord(g_nm_events[at], st);
-}
-
-static int nm_blocks(size_t count) { return (int)((count + kNmThreads - 1) / kNmThreads); }
 
 }  // namespace ma
 
@@ -268,14 +262,10 @@ extern "C" {
 
 size_t ma_estimate_normals_workspace_bytes(int n, int k) {
   if (!nm_shape_ok(n, k)) return 0;
-  return nm_layout(n, k).total;
+  return nm_buffers(n, k, nullptr).total;
 }
 
-void ma_estimate_normals_set_events(void* const* events) {
-  g_nm_timed = events != nullptr;
-  if (events)
-    for (int i = 0; i < 5; i++) g_nm_events[i] = (cudaEvent_t)events[i];
-}
+void ma_estimate_normals_set_events(void* const* events) { nm_events.set(events); }
 
 int ma_estimate_normals_last_rounds(void) { return g_nm_rounds; }
 
@@ -285,49 +275,28 @@ int ma_estimate_normals(const float* xyz, int n, int k, float* normals_out, int3
     set_error("ma_estimate_normals: bad arguments (1 <= k <= %d, k < n <= 2^24)", kKnnMaxK);
     return 1;
   }
+  const char* what = "ma_estimate_normals";
   cudaStream_t st = (cudaStream_t)stream;
-  const NmLayout L = nm_layout(n, k);
-  char* base = reinterpret_cast<char*>(ws);
-  auto* sorted = reinterpret_cast<float4*>(base + L.sorted);
-  auto* cell = reinterpret_cast<uint32_t*>(base + L.cell);
-  auto* count = reinterpret_cast<uint32_t*>(base + L.count);
-  auto* start = reinterpret_cast<uint32_t*>(base + L.start);
-  int32_t* knn = knn_out ? knn_out : reinterpret_cast<int32_t*>(base + L.knn);
-  float* uno = unoriented_out ? unoriented_out : reinterpret_cast<float*>(base + L.uno);
-  auto* w = reinterpret_cast<uint32_t*>(base + L.w);
-  auto* word = reinterpret_cast<uint32_t*>(base + L.word);
-  auto* hook = reinterpret_cast<uint32_t*>(base + L.hook);
-  auto* best1 = reinterpret_cast<unsigned long long*>(base + L.best1);
-  auto* best2 = reinterpret_cast<uint32_t*>(base + L.best2);
-  auto* hooks = reinterpret_cast<int*>(base + L.hooks);
+  NmBuffers b = nm_buffers(n, k, ws);
+  if (knn_out) b.knn = knn_out;
+  if (unoriented_out) b.uno = unoriented_out;
   const KnnGrid grid = nm_grid(n, k);
-  const int G = grid.G;
-  const size_t cells = (size_t)G * G * G, nk = (size_t)n * k;
+  const size_t nk = (size_t)n * k;
 
-  nm_mark(0, st);
-  cudaError_t e = cudaMemsetAsync(count, 0, (cells + 1) * 4, st);
-  if (e != cudaSuccess) {
-    set_error("ma_estimate_normals: %s", cudaGetErrorString(e));
-    return 1;
-  }
-  knn_cell_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(xyz, n, grid, cell, count);
-  size_t scan_bytes = nm_scan_bytes(cells);
-  e = cub::DeviceScan::ExclusiveSum(base + L.scan, scan_bytes, count, start, (int)(cells + 1), st);
-  knn_scatter_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(xyz, n, cell, start, count, sorted);
+  nm_events.mark(0, st);
+  cudaError_t e = knn_bin(xyz, n, grid, b.cell, b.count, b.start, b.sorted, b.scan, b.scan_bytes, st);
+  if (e != cudaSuccess) return stage_status(what, e);
   count_launch(3);
-  nm_mark(1, st);
+  nm_events.mark(1, st);
   knn_grid_kernel<false><<<(n + kKnnThreads - 1) / kKnnThreads, kKnnThreads,
-                           (size_t)k * kKnnThreads * sizeof(unsigned long long), st>>>(sorted, start, n, k, grid, 0,
-                                                                                       nullptr, nullptr, knn, nullptr);
-  nm_mark(2, st);
-  normals_pca_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(xyz, knn, n, k, uno);
-  nm_mark(3, st);
-  normals_weight_kernel<<<nm_blocks(nk), kNmThreads, 0, st>>>(uno, knn, n, k, w, word);
+                           (size_t)k * kKnnThreads * sizeof(unsigned long long), st>>>(b.sorted, b.start, n, k, grid, 0,
+                                                                                       nullptr, nullptr, b.knn, nullptr);
+  nm_events.mark(2, st);
+  normals_pca_kernel<<<blocks(n, kNmThreads), kNmThreads, 0, st>>>(xyz, b.knn, n, k, b.uno);
+  nm_events.mark(3, st);
+  normals_weight_kernel<<<blocks(nk, kNmThreads), kNmThreads, 0, st>>>(b.uno, b.knn, n, k, b.w, b.word);
   count_launch(3);
-  if (e != cudaSuccess || !check_launch("ma_estimate_normals")) {
-    if (e != cudaSuccess) set_error("ma_estimate_normals: %s", cudaGetErrorString(e));
-    return 1;
-  }
+  if (stage_status(what, e)) return 1;
   int rounds = 0;
   for (;;) {
     if (rounds == kNmMaxRounds) {
@@ -336,35 +305,28 @@ int ma_estimate_normals(const float* xyz, int n, int k, float* normals_out, int3
     }
     rounds++;
     int merged = 0;
-    e = cudaMemsetAsync(hooks, 0, sizeof(int), st);
-    normals_clear_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(n, best1, best2);
-    normals_min1_kernel<<<nm_blocks(nk), kNmThreads, 0, st>>>(knn, n, k, w, word, best1);
-    normals_min2_kernel<<<nm_blocks(nk), kNmThreads, 0, st>>>(knn, n, k, w, word, best1, best2);
-    normals_hook_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(uno, n, word, best1, best2, hook, hooks);
-    normals_jump_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(n, word, hook);
-    normals_relabel_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(n, hook, word);
+    e = cudaMemsetAsync(b.hooks, 0, sizeof(int), st);
+    normals_clear_kernel<<<blocks(n, kNmThreads), kNmThreads, 0, st>>>(n, b.best1, b.best2);
+    normals_min1_kernel<<<blocks(nk, kNmThreads), kNmThreads, 0, st>>>(b.knn, n, k, b.w, b.word, b.best1);
+    normals_min2_kernel<<<blocks(nk, kNmThreads), kNmThreads, 0, st>>>(b.knn, n, k, b.w, b.word, b.best1, b.best2);
+    normals_hook_kernel<<<blocks(n, kNmThreads), kNmThreads, 0, st>>>(b.uno, n, b.word, b.best1, b.best2, b.hook,
+                                                                      b.hooks);
+    normals_jump_kernel<<<blocks(n, kNmThreads), kNmThreads, 0, st>>>(n, b.word, b.hook);
+    normals_relabel_kernel<<<blocks(n, kNmThreads), kNmThreads, 0, st>>>(n, b.hook, b.word);
     count_launch(6);
-    if (e == cudaSuccess) e = cudaMemcpyAsync(&merged, hooks, sizeof(int), cudaMemcpyDeviceToHost, st);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(&merged, b.hooks, sizeof(int), cudaMemcpyDeviceToHost, st);
     if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-    if (e != cudaSuccess || !check_launch("ma_estimate_normals")) {
-      if (e != cudaSuccess) set_error("ma_estimate_normals: %s", cudaGetErrorString(e));
-      cudaGetLastError();
-      return 1;
-    }
+    if (stage_status(what, e)) return 1;
     if (merged == 0) break;
   }
   g_nm_rounds = rounds;
   // the last round hooked nothing, so best1 is free again: it collects each component's farthest point
-  e = cudaMemsetAsync(best1, 0, (size_t)n * 8, st);
-  normals_far_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(xyz, n, word, best1);
-  normals_apply_kernel<<<nm_blocks(n), kNmThreads, 0, st>>>(xyz, uno, n, word, best1, normals_out);
+  e = cudaMemsetAsync(b.best1, 0, (size_t)n * 8, st);
+  normals_far_kernel<<<blocks(n, kNmThreads), kNmThreads, 0, st>>>(xyz, n, b.word, b.best1);
+  normals_apply_kernel<<<blocks(n, kNmThreads), kNmThreads, 0, st>>>(xyz, b.uno, n, b.word, b.best1, normals_out);
   count_launch(2);
-  nm_mark(4, st);
-  if (e != cudaSuccess) {
-    set_error("ma_estimate_normals: %s", cudaGetErrorString(e));
-    return 1;
-  }
-  return check_launch("ma_estimate_normals") ? 0 : 1;
+  nm_events.mark(4, st);
+  return stage_status(what, e);
 }
 
 }  // extern "C"

@@ -25,7 +25,7 @@
 #include <cub/device/device_run_length_encode.cuh>
 #include <cub/device/device_scan.cuh>
 
-#include "internal.h"
+#include "workspace.h"
 
 namespace ma {
 
@@ -388,7 +388,6 @@ __global__ void objects_finish_kernel(int n, const ObCounters* __restrict__ ctr,
 
 // ---------------------------------------------------------------- workspace
 
-static size_t ob_align(size_t b) { return (b + 255) & ~(size_t)255; }
 static bool ob_shape_ok(int n, int min_points) { return n >= 1 && n <= kObMaxN && min_points >= 1 && min_points <= n; }
 static int ob_max_objects(int n, int min_points) { return n / min_points; }
 
@@ -419,55 +418,53 @@ static size_t ob_cub_bytes(int n, int max_objects) {
   return std::max(b, t);
 }
 
-struct ObLayout {
-  size_t ctr, key_a, key_b, val_a, val_b, ukey, runlen, start, sorted, boxes, clique, size, rank_of, objsize, okey_a,
-      okey_b, oval, cub, cub_bytes, total;
+struct ObBuffers {
+  ObCounters* ctr;
+  unsigned long long *key_a, *key_b;
+  int *val_a, *val_b;
+  unsigned long long* ukey;
+  int *runlen, *start;
+  float4 *sorted, *boxes;
+  uint8_t* clique;
+  int *size, *rank_of;
+  int64_t* objsize;
+  uint32_t *okey_a, *okey_b;
+  int64_t* oval;
+  void* cub;
+  size_t cub_bytes, total;
 };
 
-static ObLayout ob_layout(int n, int min_points) {
-  ObLayout L;
-  size_t o = 0;
-  auto take = [&](size_t bytes) { const size_t at = o; o += ob_align(bytes); return at; };
+static ObBuffers ob_buffers(int n, int min_points, void* ws) {
   const int mo = ob_max_objects(n, min_points);
-  L.ctr = take(sizeof(ObCounters));
-  L.key_a = take((size_t)n * 8);
-  L.key_b = take((size_t)n * 8);
-  L.val_a = take((size_t)n * 4);
-  L.val_b = take((size_t)n * 4);
-  L.ukey = take((size_t)n * 8);
-  L.runlen = take((size_t)(n + 1) * 4);
-  L.start = take((size_t)(n + 1) * 4);
-  L.sorted = take((size_t)n * sizeof(float4));
-  L.boxes = take((size_t)n * 2 * sizeof(float4));
-  L.clique = take((size_t)n);
-  L.size = take((size_t)n * 4);
-  L.rank_of = take((size_t)n * 4);
-  L.objsize = take((size_t)(mo + 1) * 8);
-  L.okey_a = take((size_t)n * 4);
-  L.okey_b = take((size_t)n * 4);
-  L.oval = take((size_t)n * 8);
-  L.cub_bytes = ob_cub_bytes(n, mo);
-  L.cub = take(L.cub_bytes);
-  L.total = o;
-  return L;
+  Carver c(ws);
+  ObBuffers b;
+  b.ctr = c.take<ObCounters>(1);
+  b.key_a = c.take<unsigned long long>(n);
+  b.key_b = c.take<unsigned long long>(n);
+  b.val_a = c.take<int>(n);
+  b.val_b = c.take<int>(n);
+  b.ukey = c.take<unsigned long long>(n);
+  b.runlen = c.take<int>((size_t)n + 1);
+  b.start = c.take<int>((size_t)n + 1);
+  b.sorted = c.take<float4>(n);
+  b.boxes = c.take<float4>(2 * (size_t)n);
+  b.clique = c.take<uint8_t>(n);
+  b.size = c.take<int>(n);
+  b.rank_of = c.take<int>(n);
+  b.objsize = c.take<int64_t>((size_t)mo + 1);
+  b.okey_a = c.take<uint32_t>(n);
+  b.okey_b = c.take<uint32_t>(n);
+  b.oval = c.take<int64_t>(n);
+  b.cub_bytes = ob_cub_bytes(n, mo);
+  b.cub = c.take<char>(b.cub_bytes);
+  b.total = c.total;
+  return b;
 }
 
-static cudaEvent_t g_ob_events[4];
-static bool g_ob_timed = false;
-
-static void ob_mark(int at, cudaStream_t st) {
-  if (g_ob_timed) cudaEventRecord(g_ob_events[at], st);
-}
-
-static int ob_blocks(size_t count) { return (int)((count + kObThreads - 1) / kObThreads); }
+static StageEvents<4> ob_events;
 
 // CTAs of the warp-per-cell kernels: 8 per SM, no more than one warp per point
-static int ob_warp_blocks(int n) {
-  int dev = 0, sms = 132;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-    sms = 132;
-  return std::max(1, std::min(8 * sms, ob_blocks((size_t)n * 32)));
-}
+static int ob_warp_blocks(int n) { return std::max(1, std::min(8 * sm_count(), blocks((size_t)n * 32, kObThreads))); }
 
 }  // namespace ma
 
@@ -477,14 +474,10 @@ extern "C" {
 
 size_t ma_split_objects_workspace_bytes(int n, int min_points) {
   if (!ob_shape_ok(n, min_points)) return 0;
-  return ob_layout(n, min_points).total;
+  return ob_buffers(n, min_points, nullptr).total;
 }
 
-void ma_split_objects_set_events(void* const* events) {
-  g_ob_timed = events != nullptr;
-  if (events)
-    for (int i = 0; i < 4; i++) g_ob_events[i] = (cudaEvent_t)events[i];
-}
+void ma_split_objects_set_events(void* const* events) { ob_events.set(events); }
 
 int ma_split_objects(const float* xyz, int n, float e, int min_points, int32_t* labels_out, int64_t* indices_out,
                      int64_t* offsets_out, int64_t* stats_out, void* ws, void* stream) {
@@ -495,75 +488,54 @@ int ma_split_objects(const float* xyz, int n, float e, int min_points, int32_t* 
     return 1;
   }
   cudaStream_t st = (cudaStream_t)stream;
-  const ObLayout L = ob_layout(n, min_points);
-  char* base = reinterpret_cast<char*>(ws);
-  auto* ctr = reinterpret_cast<ObCounters*>(base + L.ctr);
-  auto* key_a = reinterpret_cast<unsigned long long*>(base + L.key_a);
-  auto* key_b = reinterpret_cast<unsigned long long*>(base + L.key_b);
-  auto* val_a = reinterpret_cast<int*>(base + L.val_a);
-  auto* val_b = reinterpret_cast<int*>(base + L.val_b);
-  auto* ukey = reinterpret_cast<unsigned long long*>(base + L.ukey);
-  auto* runlen = reinterpret_cast<int*>(base + L.runlen);
-  auto* start = reinterpret_cast<int*>(base + L.start);
-  auto* sorted = reinterpret_cast<float4*>(base + L.sorted);
-  auto* boxes = reinterpret_cast<float4*>(base + L.boxes);
-  auto* clique = reinterpret_cast<uint8_t*>(base + L.clique);
-  auto* size = reinterpret_cast<int*>(base + L.size);
-  auto* rank_of = reinterpret_cast<int*>(base + L.rank_of);
-  auto* objsize = reinterpret_cast<int64_t*>(base + L.objsize);
-  auto* okey_a = reinterpret_cast<uint32_t*>(base + L.okey_a);
-  auto* okey_b = reinterpret_cast<uint32_t*>(base + L.okey_b);
-  auto* oval = reinterpret_cast<int64_t*>(base + L.oval);
-  void* tmp = base + L.cub;
-  const int mo = ob_max_objects(n, min_points), wblocks = ob_warp_blocks(n);
-  size_t tb = L.cub_bytes;
+  const ObBuffers b = ob_buffers(n, min_points, ws);
+  const int mo = ob_max_objects(n, min_points), wblocks = ob_warp_blocks(n), nb = blocks(n, kObThreads);
+  size_t tb = b.cub_bytes;
 
-  ob_mark(0, st);
-  cudaError_t e_ = cudaMemsetAsync(ctr, 0, sizeof(ObCounters), st);
-  if (e_ == cudaSuccess) e_ = cudaMemsetAsync(ctr->box, 0xff, 3 * sizeof(uint32_t), st);
-  if (e_ == cudaSuccess) e_ = cudaMemsetAsync(runlen, 0, (size_t)(n + 1) * 4, st);
-  if (e_ == cudaSuccess) e_ = cudaMemsetAsync(size, 0, (size_t)n * 4, st);
-  if (e_ == cudaSuccess) e_ = cudaMemsetAsync(objsize, 0, (size_t)(mo + 1) * 8, st);
-  objects_box_kernel<<<std::min(ob_blocks(n), 1024), kObThreads, 0, st>>>(xyz, n, ctr);
-  objects_key_kernel<<<ob_blocks(n), kObThreads, 0, st>>>(xyz, n, e, ctr, key_a, val_a);
+  ob_events.mark(0, st);
+  cudaError_t e_ = cudaMemsetAsync(b.ctr, 0, sizeof(ObCounters), st);
+  if (e_ == cudaSuccess) e_ = cudaMemsetAsync(b.ctr->box, 0xff, 3 * sizeof(uint32_t), st);
+  if (e_ == cudaSuccess) e_ = cudaMemsetAsync(b.runlen, 0, (size_t)(n + 1) * 4, st);
+  if (e_ == cudaSuccess) e_ = cudaMemsetAsync(b.size, 0, (size_t)n * 4, st);
+  if (e_ == cudaSuccess) e_ = cudaMemsetAsync(b.objsize, 0, (size_t)(mo + 1) * 8, st);
+  objects_box_kernel<<<std::min(nb, 1024), kObThreads, 0, st>>>(xyz, n, b.ctr);
+  objects_key_kernel<<<nb, kObThreads, 0, st>>>(xyz, n, e, b.ctr, b.key_a, b.val_a);
   count_launch(2);
   if (e_ == cudaSuccess)
-    e_ = cub::DeviceRadixSort::SortPairs(tmp, tb, key_a, key_b, val_a, val_b, n, 0, 3 * kObAxisBits, st);
-  tb = L.cub_bytes;
-  if (e_ == cudaSuccess) e_ = cub::DeviceRunLengthEncode::Encode(tmp, tb, key_b, ukey, runlen, &ctr->runs, n, st);
-  tb = L.cub_bytes;
-  if (e_ == cudaSuccess) e_ = cub::DeviceScan::ExclusiveSum(tmp, tb, runlen, start, n + 1, st);
-  objects_gather_kernel<<<ob_blocks(n), kObThreads, 0, st>>>(xyz, n, val_b, sorted);
-  count_launch(1);
-  ob_mark(1, st);
-  objects_cell_kernel<<<wblocks, kObThreads, 0, st>>>(sorted, start, ctr, e2, boxes, clique, labels_out);
-  objects_pair_kernel<<<wblocks, kObThreads, 0, st>>>(sorted, ukey, start, boxes, clique, ctr, e2, labels_out);
-  objects_label_kernel<<<ob_blocks(n), kObThreads, 0, st>>>(n, labels_out, size, ctr);
-  count_launch(3);
-  ob_mark(2, st);
-  objects_order_key_kernel<<<ob_blocks(n), kObThreads, 0, st>>>(n, min_points, labels_out, size, ctr, key_a);
-  count_launch(1);
-  tb = L.cub_bytes;
-  if (e_ == cudaSuccess) e_ = cub::DeviceRadixSort::SortKeysDescending(tmp, tb, key_a, key_b, n, 0, 49, st);
-  objects_rank_kernel<<<ob_blocks(n), kObThreads, 0, st>>>(n, key_b, ctr, rank_of, objsize);
-  count_launch(1);
-  tb = L.cub_bytes;
-  if (e_ == cudaSuccess) e_ = cub::DeviceScan::ExclusiveSum(tmp, tb, objsize, offsets_out, mo + 1, st);
-  objects_select_key_kernel<<<ob_blocks(n), kObThreads, 0, st>>>(n, (uint32_t)mo, labels_out, rank_of, ctr, okey_a,
-                                                                   oval);
-  count_launch(1);
-  tb = L.cub_bytes;
+    e_ = cub::DeviceRadixSort::SortPairs(b.cub, tb, b.key_a, b.key_b, b.val_a, b.val_b, n, 0, 3 * kObAxisBits, st);
+  tb = b.cub_bytes;
   if (e_ == cudaSuccess)
-    e_ = cub::DeviceRadixSort::SortPairs(tmp, tb, okey_a, okey_b, oval, indices_out, n, 0, ob_select_bits(mo), st);
-  objects_finish_kernel<<<1, 32, 0, st>>>(n, ctr, stats_out);
+    e_ = cub::DeviceRunLengthEncode::Encode(b.cub, tb, b.key_b, b.ukey, b.runlen, &b.ctr->runs, n, st);
+  tb = b.cub_bytes;
+  if (e_ == cudaSuccess) e_ = cub::DeviceScan::ExclusiveSum(b.cub, tb, b.runlen, b.start, n + 1, st);
+  objects_gather_kernel<<<nb, kObThreads, 0, st>>>(xyz, n, b.val_b, b.sorted);
   count_launch(1);
-  ob_mark(3, st);
-  if (e_ != cudaSuccess) {
-    set_error("ma_split_objects: %s", cudaGetErrorString(e_));
-    cudaGetLastError();
-    return 1;
-  }
-  return check_launch("ma_split_objects") ? 0 : 1;
+  ob_events.mark(1, st);
+  objects_cell_kernel<<<wblocks, kObThreads, 0, st>>>(b.sorted, b.start, b.ctr, e2, b.boxes, b.clique, labels_out);
+  objects_pair_kernel<<<wblocks, kObThreads, 0, st>>>(b.sorted, b.ukey, b.start, b.boxes, b.clique, b.ctr, e2,
+                                                      labels_out);
+  objects_label_kernel<<<nb, kObThreads, 0, st>>>(n, labels_out, b.size, b.ctr);
+  count_launch(3);
+  ob_events.mark(2, st);
+  objects_order_key_kernel<<<nb, kObThreads, 0, st>>>(n, min_points, labels_out, b.size, b.ctr, b.key_a);
+  count_launch(1);
+  tb = b.cub_bytes;
+  if (e_ == cudaSuccess) e_ = cub::DeviceRadixSort::SortKeysDescending(b.cub, tb, b.key_a, b.key_b, n, 0, 49, st);
+  objects_rank_kernel<<<nb, kObThreads, 0, st>>>(n, b.key_b, b.ctr, b.rank_of, b.objsize);
+  count_launch(1);
+  tb = b.cub_bytes;
+  if (e_ == cudaSuccess) e_ = cub::DeviceScan::ExclusiveSum(b.cub, tb, b.objsize, offsets_out, mo + 1, st);
+  objects_select_key_kernel<<<nb, kObThreads, 0, st>>>(n, (uint32_t)mo, labels_out, b.rank_of, b.ctr, b.okey_a,
+                                                       b.oval);
+  count_launch(1);
+  tb = b.cub_bytes;
+  if (e_ == cudaSuccess)
+    e_ = cub::DeviceRadixSort::SortPairs(b.cub, tb, b.okey_a, b.okey_b, b.oval, indices_out, n, 0, ob_select_bits(mo),
+                                         st);
+  objects_finish_kernel<<<1, 32, 0, st>>>(n, b.ctr, stats_out);
+  count_launch(1);
+  ob_events.mark(3, st);
+  return stage_status("ma_split_objects", e_);
 }
 
 }  // extern "C"

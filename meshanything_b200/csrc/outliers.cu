@@ -22,12 +22,11 @@
 #include <algorithm>
 #include <cmath>
 
-#include <cub/device/device_scan.cuh>
 #include <cub/device/device_select.cuh>
 #include <cub/iterator/counting_input_iterator.cuh>
 
-#include "internal.h"
 #include "knn_grid.cuh"
+#include "workspace.h"
 
 namespace ma {
 
@@ -251,14 +250,7 @@ __global__ void outliers_finish_kernel(const int* __restrict__ counters, const i
 
 // ---------------------------------------------------------------- workspace
 
-static size_t ol_align(size_t b) { return (b + 255) & ~(size_t)255; }
 static bool ol_shape_ok(int n, int k) { return k >= 1 && k <= kKnnMaxK && n > k && n <= kOlMaxN; }
-
-static size_t ol_scan_bytes(size_t cells) {
-  size_t bytes = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, bytes, (uint32_t*)nullptr, (uint32_t*)nullptr, (int)(cells + 1));
-  return bytes;
-}
 
 static size_t ol_occ_bytes(size_t cells) {
   size_t bytes = 0;
@@ -274,41 +266,54 @@ static size_t ol_flag_bytes(int n) {
   return bytes;
 }
 
-struct OlLayout {
-  size_t sorted, cell, count, start, scan, hist, box, ext, occ, nocc, boxes, knn, d2, dbar, part, inl, parent, size,
-      largest, counters, total;
-  size_t cub;  // bytes of the largest CUB temporary, shared by the scan and both selections
+struct OlBuffers {
+  float4* sorted;
+  uint32_t *cell, *count, *start;
+  void* cub;         // the largest CUB temporary, shared by the scan and both selections
+  size_t cub_bytes;
+  uint32_t* hist;
+  float *box, *ext;
+  uint32_t* occ;
+  int* nocc;
+  float4* boxes;
+  int32_t* knn;
+  float* d2;
+  double *dbar, *part;
+  uint8_t* inl;
+  uint32_t *parent, *size;
+  unsigned long long* largest;
+  int* counters;
+  size_t total;
 };
 
-static OlLayout ol_layout(int n, int k) {
+static OlBuffers ol_buffers(int n, int k, void* ws) {
   const int G = knn_grid_size(n, k);
   const size_t cells = (size_t)G * G * G, nk = (size_t)n * k, nbox = std::min(cells, (size_t)n);
-  OlLayout L;
-  size_t o = 0;
-  auto take = [&](size_t bytes) { const size_t at = o; o += ol_align(bytes); return at; };
-  L.cub = std::max(ol_scan_bytes(cells), std::max(ol_occ_bytes(cells), ol_flag_bytes(n)));
-  L.sorted = take((size_t)n * sizeof(float4));
-  L.cell = take((size_t)n * 4);
-  L.count = take((cells + 1) * 4);
-  L.start = take((cells + 1) * 4);
-  L.scan = take(L.cub);
-  L.hist = take(3 * kOlBins * 4);
-  L.box = take(6 * 4);
-  L.ext = take(6 * 4);
-  L.occ = take(nbox * 4);
-  L.nocc = take(4);
-  L.boxes = take(nbox * 2 * sizeof(float4));
-  L.knn = take(nk * 4);
-  L.d2 = take(nk * 4);
-  L.dbar = take((size_t)n * 8);
-  L.part = take((size_t)((n + kOlTile - 1) / kOlTile) * 8);
-  L.inl = take((size_t)n);
-  L.parent = take((size_t)n * 4);
-  L.size = take((size_t)n * 4);
-  L.largest = take(8);
-  L.counters = take(4 * 4);
-  L.total = o;
-  return L;
+  Carver c(ws);
+  OlBuffers b;
+  b.cub_bytes = std::max(knn_bin_scan_bytes(cells), std::max(ol_occ_bytes(cells), ol_flag_bytes(n)));
+  b.sorted = c.take<float4>(n);
+  b.cell = c.take<uint32_t>(n);
+  b.count = c.take<uint32_t>(cells + 1);
+  b.start = c.take<uint32_t>(cells + 1);
+  b.cub = c.take<char>(b.cub_bytes);
+  b.hist = c.take<uint32_t>(3 * kOlBins);
+  b.box = c.take<float>(6);
+  b.ext = c.take<float>(6);
+  b.occ = c.take<uint32_t>(nbox);
+  b.nocc = c.take<int>(1);
+  b.boxes = c.take<float4>(2 * nbox);
+  b.knn = c.take<int32_t>(nk);
+  b.d2 = c.take<float>(nk);
+  b.dbar = c.take<double>(n);
+  b.part = c.take<double>((n + kOlTile - 1) / kOlTile);
+  b.inl = c.take<uint8_t>(n);
+  b.parent = c.take<uint32_t>(n);
+  b.size = c.take<uint32_t>(n);
+  b.largest = c.take<unsigned long long>(1);
+  b.counters = c.take<int>(4);
+  b.total = c.total;
+  return b;
 }
 
 // the cube over the robust extent ext = (lo[3], hi[3]): its longest side (grown by kOlPad on each side) in G cells
@@ -325,24 +330,7 @@ static KnnGrid ol_grid(const float* ext, int G) {
   return g;
 }
 
-static cudaEvent_t g_ol_events[5];
-static bool g_ol_timed = false;
-
-static void ol_mark(int at, cudaStream_t st) {
-  if (g_ol_timed) cudaEventRecord(g_ol_events[at], st);
-}
-
-static int ol_blocks(size_t count) { return (int)((count + kOlThreads - 1) / kOlThreads); }
-
-static bool ol_fail(cudaError_t e) {
-  if (e != cudaSuccess) {
-    set_error("ma_remove_outliers: %s", cudaGetErrorString(e));
-    cudaGetLastError();
-    return true;
-  }
-  if (!check_launch("ma_remove_outliers")) return true;
-  return false;
-}
+static StageEvents<5> ol_events;
 
 }  // namespace ma
 
@@ -352,14 +340,10 @@ extern "C" {
 
 size_t ma_remove_outliers_workspace_bytes(int n, int k) {
   if (!ol_shape_ok(n, k)) return 0;
-  return ol_layout(n, k).total;
+  return ol_buffers(n, k, nullptr).total;
 }
 
-void ma_remove_outliers_set_events(void* const* events) {
-  g_ol_timed = events != nullptr;
-  if (events)
-    for (int i = 0; i < 5; i++) g_ol_events[i] = (cudaEvent_t)events[i];
-}
+void ma_remove_outliers_set_events(void* const* events) { ol_events.set(events); }
 
 int ma_remove_outliers(const float* xyz, int n, int k, double std_ratio, double min_component, uint8_t* keep_out,
                        int64_t* kept_idx_out, int64_t* n_kept_out, double* mean_dist_out, int32_t* knn_out,
@@ -370,77 +354,57 @@ int ma_remove_outliers(const float* xyz, int n, int k, double std_ratio, double 
               "min_component >= 0)", kKnnMaxK);
     return 1;
   }
+  const char* what = "ma_remove_outliers";
   cudaStream_t st = (cudaStream_t)stream;
-  const OlLayout L = ol_layout(n, k);
-  char* base = reinterpret_cast<char*>(ws);
-  auto* sorted = reinterpret_cast<float4*>(base + L.sorted);
-  auto* cell = reinterpret_cast<uint32_t*>(base + L.cell);
-  auto* count = reinterpret_cast<uint32_t*>(base + L.count);
-  auto* start = reinterpret_cast<uint32_t*>(base + L.start);
-  auto* hist = reinterpret_cast<uint32_t*>(base + L.hist);
-  auto* box = reinterpret_cast<float*>(base + L.box);
-  auto* ext = reinterpret_cast<float*>(base + L.ext);
-  auto* occ = reinterpret_cast<uint32_t*>(base + L.occ);
-  auto* nocc = reinterpret_cast<int*>(base + L.nocc);
-  auto* boxes = reinterpret_cast<float4*>(base + L.boxes);
-  int32_t* knn = knn_out ? knn_out : reinterpret_cast<int32_t*>(base + L.knn);
-  auto* d2 = reinterpret_cast<float*>(base + L.d2);
-  double* dbar = mean_dist_out ? mean_dist_out : reinterpret_cast<double*>(base + L.dbar);
-  auto* part = reinterpret_cast<double*>(base + L.part);
-  auto* inl = reinterpret_cast<uint8_t*>(base + L.inl);
-  auto* parent = reinterpret_cast<uint32_t*>(base + L.parent);
-  auto* size = reinterpret_cast<uint32_t*>(base + L.size);
-  auto* largest = reinterpret_cast<unsigned long long*>(base + L.largest);
-  auto* counters = reinterpret_cast<int*>(base + L.counters);
+  OlBuffers b = ol_buffers(n, k, ws);
+  if (knn_out) b.knn = knn_out;
+  if (mean_dist_out) b.dbar = mean_dist_out;
   const int G = knn_grid_size(n, k);
   const size_t cells = (size_t)G * G * G, nk = (size_t)n * k, nbox = std::min(cells, (size_t)n);
   const int tiles = (n + kOlTile - 1) / kOlTile;
-  size_t cub_bytes = L.cub;
+  size_t cub_bytes = b.cub_bytes;
 
   // (a) the robust cube: two histogram passes, the first over the whole frame [-0.5, 0.5]^3
-  ol_mark(0, st);
+  ol_events.mark(0, st);
   const float frame[6] = {-0.5f, -0.5f, -0.5f, 1.0f / kOlBins, 1.0f / kOlBins, 1.0f / kOlBins};
-  cudaError_t e = cudaMemcpyAsync(box, frame, sizeof(frame), cudaMemcpyHostToDevice, st);
-  const int hist_blocks = std::min(ol_blocks(n), 1024);
+  cudaError_t e = cudaMemcpyAsync(b.box, frame, sizeof(frame), cudaMemcpyHostToDevice, st);
+  const int hist_blocks = std::min(blocks(n, kOlThreads), 1024);
   for (int pass = 0; pass < 2 && e == cudaSuccess; pass++) {
-    e = cudaMemsetAsync(hist, 0, 3 * kOlBins * 4, st);
-    outliers_hist_kernel<<<hist_blocks, kOlThreads, 0, st>>>(xyz, n, box, hist);
-    outliers_range_kernel<<<1, 32, 0, st>>>(hist, n, pass, box, ext);
+    e = cudaMemsetAsync(b.hist, 0, 3 * kOlBins * 4, st);
+    outliers_hist_kernel<<<hist_blocks, kOlThreads, 0, st>>>(xyz, n, b.box, b.hist);
+    outliers_range_kernel<<<1, 32, 0, st>>>(b.hist, n, pass, b.box, b.ext);
     count_launch(2);
   }
   float ext_h[6];
-  if (e == cudaSuccess) e = cudaMemcpyAsync(ext_h, ext, sizeof(ext_h), cudaMemcpyDeviceToHost, st);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(ext_h, b.ext, sizeof(ext_h), cudaMemcpyDeviceToHost, st);
   if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-  if (ol_fail(e)) return 1;
+  if (stage_status(what, e)) return 1;
   const KnnGrid grid = ol_grid(ext_h, G);
-  e = cudaMemsetAsync(count, 0, (cells + 1) * 4, st);
-  knn_cell_kernel<<<ol_blocks(n), kOlThreads, 0, st>>>(xyz, n, grid, cell, count);
-  if (e == cudaSuccess) e = cub::DeviceScan::ExclusiveSum(base + L.scan, cub_bytes, count, start, (int)(cells + 1), st);
-  knn_scatter_kernel<<<ol_blocks(n), kOlThreads, 0, st>>>(xyz, n, cell, start, count, sorted);
-  cub_bytes = L.cub;
-  if (e == cudaSuccess)
-    e = cub::DeviceSelect::If(base + L.scan, cub_bytes, cub::CountingInputIterator<uint32_t>(0), occ, nocc, (int)cells,
-                              OlOccupied{start}, st);
-  outliers_box_kernel<<<ol_blocks(nbox), kOlThreads, 0, st>>>(sorted, start, occ, nocc, boxes);
+  e = knn_bin(xyz, n, grid, b.cell, b.count, b.start, b.sorted, b.cub, cub_bytes, st);
+  if (e != cudaSuccess) return stage_status(what, e);
+  e = cub::DeviceSelect::If(b.cub, cub_bytes, cub::CountingInputIterator<uint32_t>(0), b.occ, b.nocc, (int)cells,
+                            OlOccupied{b.start}, st);
+  outliers_box_kernel<<<blocks(nbox, kOlThreads), kOlThreads, 0, st>>>(b.sorted, b.start, b.occ, b.nocc, b.boxes);
   count_launch(3);
-  ol_mark(1, st);
+  ol_events.mark(1, st);
   // (b) kNN with the fp32 d^2 of every neighbour
   knn_grid_kernel<true><<<(n + kKnnThreads - 1) / kKnnThreads, kKnnThreads,
-                          (size_t)k * kKnnThreads * sizeof(unsigned long long), st>>>(sorted, start, n, k, grid,
-                                                                                      kOlBudget, boxes, nocc, knn, d2);
+                          (size_t)k * kKnnThreads * sizeof(unsigned long long), st>>>(
+      b.sorted, b.start, n, k, grid, kOlBudget, b.boxes, b.nocc, b.knn, b.d2);
   count_launch(1);
-  ol_mark(2, st);
+  ol_events.mark(2, st);
   // (c) mean distances, mu, sigma, the statistical inliers
-  if (e == cudaSuccess) e = cudaMemsetAsync(counters, 0, 4 * 4, st);
-  outliers_mean_kernel<<<ol_blocks(n), kOlThreads, 0, st>>>(d2, n, k, dbar);
-  outliers_tile_kernel<<<tiles, kOlTile, 0, st>>>(dbar, n, nullptr, part);
-  outliers_moment_kernel<<<1, 32, 0, st>>>(part, tiles, n, 0, std_ratio, stats_out);
-  outliers_tile_kernel<<<tiles, kOlTile, 0, st>>>(dbar, n, stats_out, part);
-  outliers_moment_kernel<<<1, 32, 0, st>>>(part, tiles, n, 1, std_ratio, stats_out);
-  outliers_inlier_kernel<<<ol_blocks(n), kOlThreads, 0, st>>>(dbar, n, stats_out, inl, parent, counters);
+  if (e == cudaSuccess) e = cudaMemsetAsync(b.counters, 0, 4 * 4, st);
+  outliers_mean_kernel<<<blocks(n, kOlThreads), kOlThreads, 0, st>>>(b.d2, n, k, b.dbar);
+  outliers_tile_kernel<<<tiles, kOlTile, 0, st>>>(b.dbar, n, nullptr, b.part);
+  outliers_moment_kernel<<<1, 32, 0, st>>>(b.part, tiles, n, 0, std_ratio, stats_out);
+  outliers_tile_kernel<<<tiles, kOlTile, 0, st>>>(b.dbar, n, stats_out, b.part);
+  outliers_moment_kernel<<<1, 32, 0, st>>>(b.part, tiles, n, 1, std_ratio, stats_out);
+  outliers_inlier_kernel<<<blocks(n, kOlThreads), kOlThreads, 0, st>>>(b.dbar, n, stats_out, b.inl, b.parent,
+                                                                       b.counters);
   count_launch(6);
-  ol_mark(3, st);
-  if (ol_fail(e)) return 1;
+  ol_events.mark(3, st);
+  if (stage_status(what, e)) return 1;
   // (d) components of the inlier graph (skipped when min_component = 0: every inlier is kept)
   int rounds = 0;
   if (min_component > 0.0) {
@@ -451,33 +415,35 @@ int ma_remove_outliers(const float* xyz, int n, int k, double std_ratio, double 
       }
       rounds++;
       int changed = 0;
-      e = cudaMemsetAsync(counters + 3, 0, 4, st);
-      outliers_hook_kernel<<<ol_blocks(nk), kOlThreads, 0, st>>>(knn, n, k, inl, parent, counters + 3);
-      outliers_jump_kernel<<<ol_blocks(n), kOlThreads, 0, st>>>(n, parent);
+      e = cudaMemsetAsync(b.counters + 3, 0, 4, st);
+      outliers_hook_kernel<<<blocks(nk, kOlThreads), kOlThreads, 0, st>>>(b.knn, n, k, b.inl, b.parent,
+                                                                          b.counters + 3);
+      outliers_jump_kernel<<<blocks(n, kOlThreads), kOlThreads, 0, st>>>(n, b.parent);
       count_launch(2);
-      if (e == cudaSuccess) e = cudaMemcpyAsync(&changed, counters + 3, 4, cudaMemcpyDeviceToHost, st);
+      if (e == cudaSuccess) e = cudaMemcpyAsync(&changed, b.counters + 3, 4, cudaMemcpyDeviceToHost, st);
       if (e == cudaSuccess) e = cudaStreamSynchronize(st);
-      if (ol_fail(e)) return 1;
+      if (stage_status(what, e)) return 1;
       if (changed == 0) break;
     }
-    e = cudaMemsetAsync(size, 0, (size_t)n * 4, st);
-    if (e == cudaSuccess) e = cudaMemsetAsync(largest, 0, 8, st);
-    outliers_size_kernel<<<ol_blocks(n), kOlThreads, 0, st>>>(n, inl, parent, size);
-    outliers_largest_kernel<<<ol_blocks(n), kOlThreads, 0, st>>>(n, inl, parent, size, largest, counters);
-    outliers_keep_kernel<<<ol_blocks(n), kOlThreads, 0, st>>>(n, inl, parent, size, largest, min_component, counters,
-                                                              keep_out);
+    e = cudaMemsetAsync(b.size, 0, (size_t)n * 4, st);
+    if (e == cudaSuccess) e = cudaMemsetAsync(b.largest, 0, 8, st);
+    outliers_size_kernel<<<blocks(n, kOlThreads), kOlThreads, 0, st>>>(n, b.inl, b.parent, b.size);
+    outliers_largest_kernel<<<blocks(n, kOlThreads), kOlThreads, 0, st>>>(n, b.inl, b.parent, b.size, b.largest,
+                                                                          b.counters);
+    outliers_keep_kernel<<<blocks(n, kOlThreads), kOlThreads, 0, st>>>(n, b.inl, b.parent, b.size, b.largest,
+                                                                       min_component, b.counters, keep_out);
     count_launch(3);
   } else if (e == cudaSuccess) {
-    e = cudaMemcpyAsync(keep_out, inl, (size_t)n, cudaMemcpyDeviceToDevice, st);
+    e = cudaMemcpyAsync(keep_out, b.inl, (size_t)n, cudaMemcpyDeviceToDevice, st);
   }
-  cub_bytes = L.cub;
+  cub_bytes = b.cub_bytes;
   if (e == cudaSuccess)
-    e = cub::DeviceSelect::Flagged(base + L.scan, cub_bytes, cub::CountingInputIterator<int64_t>(0), keep_out,
-                                   kept_idx_out, n_kept_out, n, st);
-  outliers_finish_kernel<<<1, 32, 0, st>>>(counters, n_kept_out, rounds, stats_out);
+    e = cub::DeviceSelect::Flagged(b.cub, cub_bytes, cub::CountingInputIterator<int64_t>(0), keep_out, kept_idx_out,
+                                   n_kept_out, n, st);
+  outliers_finish_kernel<<<1, 32, 0, st>>>(b.counters, n_kept_out, rounds, stats_out);
   count_launch(1);
-  ol_mark(4, st);
-  return ol_fail(e) ? 1 : 0;
+  ol_events.mark(4, st);
+  return stage_status(what, e);
 }
 
 }  // extern "C"

@@ -24,9 +24,9 @@
 #include <cub/device/device_select.cuh>
 #include <cub/iterator/counting_input_iterator.cuh>
 
-#include "internal.h"
 #include "jacobi3.cuh"
 #include "philox.cuh"
+#include "workspace.h"
 
 namespace ma {
 
@@ -264,7 +264,6 @@ __global__ void plane_finish_kernel(const PlCounters* __restrict__ ctr, const fl
 
 // ---------------------------------------------------------------- workspace
 
-static size_t pl_align(size_t b) { return (b + 255) & ~(size_t)255; }
 static bool pl_shape_ok(int n, int h) { return n >= 3 && n <= kPlMaxN && h >= 1 && h <= kPlMaxH; }
 static int pl_tiles(int n) { return (n + kPlTile - 1) / kPlTile; }
 
@@ -275,42 +274,39 @@ static size_t pl_flag_bytes(int n) {
   return bytes;
 }
 
-struct PlLayout {
-  size_t planes, counts, ctr, cls, part, cent, fit, cub, total;
+struct PlBuffers {
+  float4* planes;
+  int* counts;
+  PlCounters* ctr;
+  uint8_t* cls;
+  double *part, *cent;
+  float4* fit;
+  void* cub;
+  size_t cub_bytes, total;
 };
 
-static PlLayout pl_layout(int n, int h) {
-  PlLayout L;
-  size_t o = 0;
-  auto take = [&](size_t bytes) { const size_t at = o; o += pl_align(bytes); return at; };
-  L.planes = take((size_t)h * sizeof(float4));
-  L.counts = take((size_t)h * 4);
-  L.ctr = take(sizeof(PlCounters));
-  L.cls = take((size_t)n);
-  L.part = take((size_t)pl_tiles(n) * 6 * 8);
-  L.cent = take(3 * 8);
-  L.fit = take(sizeof(float4));
-  L.cub = take(pl_flag_bytes(n));
-  L.total = o;
-  return L;
+static PlBuffers pl_buffers(int n, int h, void* ws) {
+  Carver c(ws);
+  PlBuffers b;
+  b.planes = c.take<float4>(h);
+  b.counts = c.take<int>(h);
+  b.ctr = c.take<PlCounters>(1);
+  b.cls = c.take<uint8_t>(n);
+  b.part = c.take<double>((size_t)pl_tiles(n) * 6);
+  b.cent = c.take<double>(3);
+  b.fit = c.take<float4>(1);
+  b.cub_bytes = pl_flag_bytes(n);
+  b.cub = c.take<char>(b.cub_bytes);
+  b.total = c.total;
+  return b;
 }
 
-static cudaEvent_t g_pl_events[5];
-static bool g_pl_timed = false;
-
-static void pl_mark(int at, cudaStream_t st) {
-  if (g_pl_timed) cudaEventRecord(g_pl_events[at], st);
-}
-
-static int pl_blocks(size_t count) { return (int)((count + kPlThreads - 1) / kPlThreads); }
+static StageEvents<5> pl_events;
 
 // point slices of the scoring grid: about four CTAs per SM over all plane groups, at most one per stage of points
 static int pl_score_slices(int n, int groups) {
-  int dev = 0, sms = 132;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-    sms = 132;
   const int stages = (n + kPlPoints - 1) / kPlPoints;
-  return std::max(1, std::min(stages, (4 * sms + groups - 1) / groups));
+  return std::max(1, std::min(stages, (4 * sm_count() + groups - 1) / groups));
 }
 
 }  // namespace ma
@@ -321,14 +317,10 @@ extern "C" {
 
 size_t ma_remove_plane_workspace_bytes(int n, int h) {
   if (!pl_shape_ok(n, h)) return 0;
-  return pl_layout(n, h).total;
+  return pl_buffers(n, h, nullptr).total;
 }
 
-void ma_remove_plane_set_events(void* const* events) {
-  g_pl_timed = events != nullptr;
-  if (events)
-    for (int i = 0; i < 5; i++) g_pl_events[i] = (cudaEvent_t)events[i];
-}
+void ma_remove_plane_set_events(void* const* events) { pl_events.set(events); }
 
 int ma_remove_plane(const float* xyz, int n, int h, float t, unsigned long long seed, uint8_t* keep_out,
                     int64_t* kept_idx_out, int64_t* n_kept_out, int32_t* counts_out, float* planes_out,
@@ -339,48 +331,37 @@ int ma_remove_plane(const float* xyz, int n, int h, float t, unsigned long long 
     return 1;
   }
   cudaStream_t st = (cudaStream_t)stream;
-  const PlLayout L = pl_layout(n, h);
-  char* base = reinterpret_cast<char*>(ws);
-  float4* planes = planes_out ? reinterpret_cast<float4*>(planes_out) : reinterpret_cast<float4*>(base + L.planes);
-  int* counts = counts_out ? counts_out : reinterpret_cast<int*>(base + L.counts);
-  auto* ctr = reinterpret_cast<PlCounters*>(base + L.ctr);
-  auto* cls = reinterpret_cast<uint8_t*>(base + L.cls);
-  auto* part = reinterpret_cast<double*>(base + L.part);
-  auto* cent = reinterpret_cast<double*>(base + L.cent);
-  auto* fit = reinterpret_cast<float4*>(base + L.fit);
+  PlBuffers b = pl_buffers(n, h, ws);
+  if (planes_out) b.planes = reinterpret_cast<float4*>(planes_out);
+  if (counts_out) b.counts = counts_out;
   const int tiles = pl_tiles(n), groups = (h + kPlPlanes - 1) / kPlPlanes;
-  size_t cub_bytes = pl_flag_bytes(n);
 
-  pl_mark(0, st);
-  cudaError_t e = cudaMemsetAsync(ctr, 0, sizeof(PlCounters), st);
-  if (e == cudaSuccess) e = cudaMemsetAsync(counts, 0, (size_t)h * 4, st);
-  plane_hypothesis_kernel<<<pl_blocks(h), kPlThreads, 0, st>>>(xyz, n, h, seed, planes, ctr);
+  pl_events.mark(0, st);
+  cudaError_t e = cudaMemsetAsync(b.ctr, 0, sizeof(PlCounters), st);
+  if (e == cudaSuccess) e = cudaMemsetAsync(b.counts, 0, (size_t)h * 4, st);
+  plane_hypothesis_kernel<<<blocks(h, kPlThreads), kPlThreads, 0, st>>>(xyz, n, h, seed, b.planes, b.ctr);
   count_launch(1);
-  pl_mark(1, st);
-  plane_score_kernel<<<dim3(pl_score_slices(n, groups), groups), kPlThreads, 0, st>>>(xyz, n, h, t, planes, counts);
-  plane_winner_kernel<<<pl_blocks(h), kPlThreads, 0, st>>>(counts, h, ctr);
+  pl_events.mark(1, st);
+  plane_score_kernel<<<dim3(pl_score_slices(n, groups), groups), kPlThreads, 0, st>>>(xyz, n, h, t, b.planes,
+                                                                                        b.counts);
+  plane_winner_kernel<<<blocks(h, kPlThreads), kPlThreads, 0, st>>>(b.counts, h, b.ctr);
   count_launch(2);
-  pl_mark(2, st);
-  plane_tile_kernel<<<tiles, kPlTile, 0, st>>>(xyz, n, t, planes, ctr, cent, 0, part);
-  plane_reduce_kernel<<<1, 32, 0, st>>>(part, tiles, ctr, 0, cent, fit);
-  plane_tile_kernel<<<tiles, kPlTile, 0, st>>>(xyz, n, t, planes, ctr, cent, 1, part);
-  plane_reduce_kernel<<<1, 32, 0, st>>>(part, tiles, ctr, 1, cent, fit);
+  pl_events.mark(2, st);
+  plane_tile_kernel<<<tiles, kPlTile, 0, st>>>(xyz, n, t, b.planes, b.ctr, b.cent, 0, b.part);
+  plane_reduce_kernel<<<1, 32, 0, st>>>(b.part, tiles, b.ctr, 0, b.cent, b.fit);
+  plane_tile_kernel<<<tiles, kPlTile, 0, st>>>(xyz, n, t, b.planes, b.ctr, b.cent, 1, b.part);
+  plane_reduce_kernel<<<1, 32, 0, st>>>(b.part, tiles, b.ctr, 1, b.cent, b.fit);
   count_launch(4);
-  pl_mark(3, st);
-  plane_classify_kernel<<<pl_blocks(n), kPlThreads, 0, st>>>(xyz, n, t, fit, ctr, cls);
-  plane_keep_kernel<<<pl_blocks(n), kPlThreads, 0, st>>>(n, ctr, cls, keep_out);
+  pl_events.mark(3, st);
+  plane_classify_kernel<<<blocks(n, kPlThreads), kPlThreads, 0, st>>>(xyz, n, t, b.fit, b.ctr, b.cls);
+  plane_keep_kernel<<<blocks(n, kPlThreads), kPlThreads, 0, st>>>(n, b.ctr, b.cls, keep_out);
   if (e == cudaSuccess)
-    e = cub::DeviceSelect::Flagged(base + L.cub, cub_bytes, cub::CountingInputIterator<int64_t>(0), keep_out,
-                                   kept_idx_out, n_kept_out, n, st);
-  plane_finish_kernel<<<1, 32, 0, st>>>(ctr, fit, n_kept_out, stats_out);
+    e = cub::DeviceSelect::Flagged(b.cub, b.cub_bytes, cub::CountingInputIterator<int64_t>(0), keep_out, kept_idx_out,
+                                   n_kept_out, n, st);
+  plane_finish_kernel<<<1, 32, 0, st>>>(b.ctr, b.fit, n_kept_out, stats_out);
   count_launch(3);
-  pl_mark(4, st);
-  if (e != cudaSuccess) {
-    set_error("ma_remove_plane: %s", cudaGetErrorString(e));
-    cudaGetLastError();
-    return 1;
-  }
-  return check_launch("ma_remove_plane") ? 0 : 1;
+  pl_events.mark(4, st);
+  return stage_status("ma_remove_plane", e);
 }
 
 }  // extern "C"

@@ -20,7 +20,7 @@
 #include <algorithm>
 #include <cmath>
 
-#include "internal.h"
+#include "workspace.h"
 
 namespace cg = cooperative_groups;
 
@@ -114,8 +114,22 @@ __global__ void __launch_bounds__(kFpsThreads, 1)
 
 // ---------------------------------------------------------------- host
 
-static size_t fps_align(size_t b) { return (b + 255) & ~(size_t)255; }
 static bool fps_shape_ok(int n, int m) { return n >= 1 && n <= kFpsMaxN && m >= 1 && m <= n; }
+
+struct FpsBuffers {
+  unsigned long long* slots;  // one per pick
+  float* soa;                 // x | y | z | D of the global-memory path
+  size_t total;
+};
+
+static FpsBuffers fps_buffers(int n, int m, void* ws) {
+  Carver c(ws);
+  FpsBuffers b;
+  b.slots = c.take<unsigned long long>(m);
+  b.soa = c.take<float>(4 * (size_t)n);
+  b.total = c.total;
+  return b;
+}
 
 static int g_fps_force = kFpsAuto;
 static int g_fps_last = 0;
@@ -204,7 +218,7 @@ extern "C" {
 
 size_t ma_farthest_point_sample_workspace_bytes(int n, int m) {
   if (!fps_shape_ok(n, m)) return 0;
-  return fps_align((size_t)m * 8) + fps_align((size_t)n * 16);
+  return fps_buffers(n, m, nullptr).total;
 }
 
 int ma_farthest_point_sample_set_path(int path) {
@@ -224,26 +238,21 @@ int ma_farthest_point_sample(const float* xyz, int n, int m, int start, int64_t*
   FpsPlan p;
   if (!fps_plan(n, &p)) return 1;
   cudaStream_t st = (cudaStream_t)stream;
-  auto* slots = reinterpret_cast<unsigned long long*>(ws);
-  auto* soa = reinterpret_cast<float*>(reinterpret_cast<char*>(ws) + fps_align((size_t)m * 8));
+  FpsBuffers b = fps_buffers(n, m, ws);
   cudaError_t e = cudaSuccess;
   if (p.path == kFpsOneCta) {
-    fps_kernel<false, true><<<1, kFpsThreads, p.smem, st>>>(xyz, n, m, start, p.slice, soa, slots, out_idx, out_r2);
+    fps_kernel<false, true><<<1, kFpsThreads, p.smem, st>>>(xyz, n, m, start, p.slice, b.soa, b.slots, out_idx,
+                                                            out_r2);
   } else {
-    e = cudaMemsetAsync(slots, 0, (size_t)m * 8, st);
-    void* args[] = {(void*)&xyz, &n, &m, &start, &p.slice, &soa, &slots, &out_idx, &out_r2};
+    e = cudaMemsetAsync(b.slots, 0, (size_t)m * 8, st);
+    void* args[] = {(void*)&xyz, &n, &m, &start, &p.slice, &b.soa, &b.slots, &out_idx, &out_r2};
     if (e == cudaSuccess)
       e = cudaLaunchCooperativeKernel(p.path == kFpsGridShared ? (const void*)fps_kernel<true, true>
                                                                : (const void*)fps_kernel<true, false>,
                                       dim3(p.blocks), dim3(kFpsThreads), args, p.smem, st);
   }
   count_launch(1);
-  if (e != cudaSuccess) {
-    set_error("ma_farthest_point_sample: %s", cudaGetErrorString(e));
-    cudaGetLastError();
-    return 1;
-  }
-  if (!check_launch("ma_farthest_point_sample")) return 1;
+  if (stage_status("ma_farthest_point_sample", e)) return 1;
   g_fps_last = p.path;
   return 0;
 }

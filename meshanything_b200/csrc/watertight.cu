@@ -17,9 +17,9 @@
 #include <cub/device/device_scan.cuh>
 
 #include "canon.cuh"
-#include "internal.h"
 #include "mc_table.h"
 #include "tri_dist.cuh"
+#include "workspace.h"
 
 namespace ma {
 
@@ -136,8 +136,6 @@ __global__ void mc_emit_kernel(const float* __restrict__ field, int n, float lev
   }
 }
 
-static size_t mc_align(size_t b) { return (b + 255) & ~(size_t)255; }
-
 static size_t mc_scan_bytes(int n) {
   size_t bytes = 0;
   cub::DeviceScan::ExclusiveSum(nullptr, bytes, (unsigned long long*)nullptr, (int)((size_t)n * n * n));
@@ -172,7 +170,7 @@ int ma_udf_grid(const float* vertices, const int32_t* faces, int n_faces, int n,
 size_t ma_marching_cubes_workspace_bytes(int n) {
   if (n < 2 || n > 1024) return 0;
   const size_t N = (size_t)n * n * n;
-  return mc_align(N * sizeof(unsigned long long)) + mc_align(N * sizeof(uint16_t)) + mc_align(mc_scan_bytes(n));
+  return ws_align(N * sizeof(unsigned long long)) + ws_align(N * sizeof(uint16_t)) + ws_align(mc_scan_bytes(n));
 }
 
 int ma_marching_cubes_count(const float* field, int n, float level, void* ws, int64_t* counts_host, void* stream) {
@@ -184,8 +182,8 @@ int ma_marching_cubes_count(const float* field, int n, float level, void* ws, in
   const size_t N = (size_t)n * n * n;
   char* w = reinterpret_cast<char*>(ws);
   auto* cnt = reinterpret_cast<unsigned long long*>(w);
-  auto* info = reinterpret_cast<uint16_t*>(w + mc_align(N * sizeof(unsigned long long)));
-  void* tmp = w + mc_align(N * sizeof(unsigned long long)) + mc_align(N * sizeof(uint16_t));
+  auto* info = reinterpret_cast<uint16_t*>(w + ws_align(N * sizeof(unsigned long long)));
+  void* tmp = w + ws_align(N * sizeof(unsigned long long)) + ws_align(N * sizeof(uint16_t));
   size_t tmp_bytes = mc_scan_bytes(n);
   mc_classify_kernel<<<grid_blocks(N), 256, 0, st>>>(field, n, level, info, cnt);
   count_launch();
@@ -220,7 +218,7 @@ int ma_marching_cubes_emit(const float* field, int n, float level, const void* w
   const size_t N = (size_t)n * n * n;
   const char* w = reinterpret_cast<const char*>(ws);
   const auto* off = reinterpret_cast<const unsigned long long*>(w);
-  const auto* info = reinterpret_cast<const uint16_t*>(w + mc_align(N * sizeof(unsigned long long)));
+  const auto* info = reinterpret_cast<const uint16_t*>(w + ws_align(N * sizeof(unsigned long long)));
   mc_emit_kernel<<<grid_blocks(N), 256, 0, (cudaStream_t)stream>>>(field, n, level, info, off, out_vertices, out_faces);
   count_launch();
   return check_launch("ma_marching_cubes_emit") ? 0 : 1;

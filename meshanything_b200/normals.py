@@ -12,21 +12,10 @@ There is no CPU fallback.
 """
 from __future__ import annotations
 
-import numpy as np
 import torch
 
-from . import capi, metrics
-
-
-def _device() -> torch.device:
-    if not torch.cuda.is_available():
-        raise RuntimeError("estimating normals (--input_type pc) needs a CUDA GPU and libmeshanything_b200.so; there is "
-                           "no CPU fallback (clouds with normals go through --input_type pc_normal)")
-    try:
-        capi.lib()
-    except Exception as e:
-        raise RuntimeError("estimating normals (--input_type pc) needs libmeshanything_b200.so: " + str(e)) from e
-    return torch.device("cuda", torch.cuda.current_device())
+from . import capi
+from .pointcloud import frame_points, require_gpu
 
 
 def estimate_normals(points, k: int = 16) -> torch.Tensor:
@@ -34,14 +23,6 @@ def estimate_normals(points, k: int = 16) -> torch.Tensor:
 
     float64 input is first shifted by its float64 bounding-box centre, so large offsets (scan or UTM coordinates) do not
     cost precision in the fp32 frame; fp32 / fp16 input goes through the frame map as it is."""
-    dev = _device()
-    pts = torch.as_tensor(np.asarray(points) if not isinstance(points, torch.Tensor) else points)
-    if pts.dim() != 2 or pts.shape[1] != 3:
-        raise ValueError(f"estimate_normals: points [N, 3], got {tuple(pts.shape)}")
-    if not pts.is_floating_point():
-        pts = pts.to(torch.float64)
-    pts = pts.to(dev)
-    if pts.dtype == torch.float64 and pts.shape[0] > 0:
-        pts = pts - (pts.amin(dim=0) + pts.amax(dim=0)) / 2
-    frame = metrics.to_output_frame(pts[None])[0]
-    return capi.estimate_normals(frame, k)
+    dev = require_gpu("estimating normals (--input_type pc)",
+                      " (clouds with normals go through --input_type pc_normal)")
+    return capi.estimate_normals(frame_points(points, dev, "estimate_normals"), k)

@@ -14,11 +14,9 @@ from __future__ import annotations
 from typing import NamedTuple
 
 import numpy as np
-import torch
 
 from . import capi
-from .outliers import frame_points
-from .plane import _longest_side
+from .pointcloud import frame_points, longest_side, require_gpu
 
 
 class ObjectStats(NamedTuple):
@@ -32,30 +30,15 @@ class ObjectStats(NamedTuple):
     distance: float               # e in the input's own units
 
 
-def _device() -> torch.device:
-    if not torch.cuda.is_available():
-        raise RuntimeError("splitting a cloud into objects (--split_objects) needs a CUDA GPU and "
-                           "libmeshanything_b200.so; there is no CPU fallback")
-    try:
-        capi.lib()
-    except Exception as e:
-        raise RuntimeError("splitting a cloud into objects (--split_objects) needs libmeshanything_b200.so: " + str(e)) from e
-    return torch.device("cuda", torch.cuda.current_device())
-
-
 def split_objects(points, distance: float = 0.02, min_points: int = 4096):
     """points [N, 3] -> (object indices int64 on the GPU, offsets int64 [objects + 1] on the GPU, ObjectStats).
 
     Object k holds indices[offsets[k]:offsets[k + 1]], ascending.  distance the neighbour distance as a share of the
     bounding box's longest side (0 < distance <= 1), 1 <= min_points <= N, 1 <= N <= 2^24."""
-    dev = _device()
-    shape = tuple(points.shape) if hasattr(points, "shape") else np.shape(points)
-    if len(shape) != 2 or shape[1] != 3:
-        raise ValueError(f"split_objects: points [N, 3], got {shape}")
-    frame = frame_points(points, dev).contiguous()
-    _, idx, offsets, st = capi.split_objects(frame, distance, min_points)
+    dev = require_gpu("splitting a cloud into objects (--split_objects)")
+    _, idx, offsets, st = capi.split_objects(frame_points(points, dev, "split_objects"), distance, min_points)
     off = offsets.cpu().numpy()
     return idx, offsets, ObjectStats(clusters=int(st[0]), objects=int(st[1]), object_points=int(st[2]),
                                      dropped_clusters=int(st[3]), dropped_points=int(st[4]),
                                      largest_dropped=int(st[5]), sizes=tuple(int(x) for x in np.diff(off)),
-                                     distance=float(np.float32(distance)) * _longest_side(points))
+                                     distance=float(np.float32(distance)) * longest_side(points))

@@ -13,10 +13,8 @@ from __future__ import annotations
 
 from typing import NamedTuple
 
-import numpy as np
-import torch
-
-from . import capi, metrics
+from . import capi
+from .pointcloud import frame_points, require_gpu
 
 
 class OutlierStats(NamedTuple):
@@ -31,38 +29,13 @@ class OutlierStats(NamedTuple):
     kept: int
 
 
-def _device() -> torch.device:
-    if not torch.cuda.is_available():
-        raise RuntimeError("removing outliers (--remove_outliers) needs a CUDA GPU and libmeshanything_b200.so; there is "
-                           "no CPU fallback")
-    try:
-        capi.lib()
-    except Exception as e:
-        raise RuntimeError("removing outliers (--remove_outliers) needs libmeshanything_b200.so: " + str(e)) from e
-    return torch.device("cuda", torch.cuda.current_device())
-
-
-def frame_points(points, dev) -> torch.Tensor:
-    """[N, 3] (numpy or torch, any float dtype) -> fp32 [N, 3] in the output frame on `dev`; float64 input is first
-    shifted by its float64 bounding-box centre (as normals.estimate_normals does)."""
-    pts = torch.as_tensor(np.asarray(points) if not isinstance(points, torch.Tensor) else points)
-    if pts.dim() != 2 or pts.shape[1] != 3:
-        raise ValueError(f"remove_outliers: points [N, 3], got {tuple(pts.shape)}")
-    if not pts.is_floating_point():
-        pts = pts.to(torch.float64)
-    pts = pts.to(dev)
-    if pts.dtype == torch.float64 and pts.shape[0] > 0:
-        pts = pts - (pts.amin(dim=0) + pts.amax(dim=0)) / 2
-    return metrics.to_output_frame(pts[None])[0]
-
-
 def remove_outliers(points, k: int = 16, std_ratio: float = 2.0, min_component: float = 0.01):
     """points [N, 3] -> (kept indices int64 [n_kept], ascending, on the GPU; OutlierStats).
 
     k neighbours (1..64, k < N), std_ratio the distance threshold in standard deviations above the mean,
     min_component the least share of the statistical inliers a connected component must hold (0: keep all)."""
-    dev = _device()
-    idx, keep, st = capi.remove_outliers(frame_points(points, dev), k, std_ratio, min_component)
+    dev = require_gpu("removing outliers (--remove_outliers)")
+    idx, keep, st = capi.remove_outliers(frame_points(points, dev, "remove_outliers"), k, std_ratio, min_component)
     n, inl, kept = keep.shape[0], int(st[3]), int(st[6])
     return idx, OutlierStats(n_points=n, removed_statistical=n - inl, removed_components=inl - kept,
                              components=int(st[4]), components_dropped=int(st[5]), mean_distance=float(st[0]),

@@ -15,10 +15,9 @@ from __future__ import annotations
 from typing import NamedTuple
 
 import numpy as np
-import torch
 
 from . import capi
-from .outliers import frame_points
+from .pointcloud import frame_points, longest_side, require_gpu
 
 
 class PlaneStats(NamedTuple):
@@ -35,38 +34,15 @@ class PlaneStats(NamedTuple):
     kept: int
 
 
-def _device() -> torch.device:
-    if not torch.cuda.is_available():
-        raise RuntimeError("removing the support plane (--remove_plane) needs a CUDA GPU and libmeshanything_b200.so; "
-                           "there is no CPU fallback")
-    try:
-        capi.lib()
-    except Exception as e:
-        raise RuntimeError("removing the support plane (--remove_plane) needs libmeshanything_b200.so: " + str(e)) from e
-    return torch.device("cuda", torch.cuda.current_device())
-
-
-def _longest_side(points) -> float:
-    """The longest side of the bounding box in the input's units (the length the frame divides by; 0 counts as 1)."""
-    pts = points if isinstance(points, torch.Tensor) else torch.as_tensor(np.asarray(points))
-    pts = pts.to(torch.float64)
-    side = float((pts.amax(dim=0) - pts.amin(dim=0)).max()) if pts.shape[0] else 0.0
-    return side if side > 0 else 1.0
-
-
 def remove_plane(points, distance: float = 0.01, iterations: int = 1000, seed: int = 0):
     """points [N, 3] -> (kept indices int64 [n_kept], ascending, on the GPU; PlaneStats).
 
     distance the on-plane threshold as a share of the bounding box's longest side (0 < distance <= 1), iterations the
     number of RANSAC hypotheses (1..65536), seed any integer in [0, 2^64).  3 <= N <= 2^24."""
-    dev = _device()
-    shape = tuple(points.shape) if hasattr(points, "shape") else np.shape(points)
-    if len(shape) != 2 or shape[1] != 3:
-        raise ValueError(f"remove_plane: points [N, 3], got {shape}")
-    frame = frame_points(points, dev).contiguous()
-    idx, keep, st = capi.remove_plane(frame, distance, iterations, seed)
+    dev = require_gpu("removing the support plane (--remove_plane)")
+    idx, keep, st = capi.remove_plane(frame_points(points, dev, "remove_plane"), distance, iterations, seed)
     t32 = float(np.float32(distance))
     return idx, PlaneStats(found=bool(st[0]), normal=(float(st[1]), float(st[2]), float(st[3])), offset=float(st[4]),
-                           threshold=t32 * _longest_side(points), hypothesis=int(st[5]), hypothesis_count=int(st[6]),
+                           threshold=t32 * longest_side(points), hypothesis=int(st[5]), hypothesis_count=int(st[6]),
                            valid_hypotheses=int(st[7]), on=int(st[8]), above=int(st[9]), below=int(st[10]),
                            kept=int(st[11]))

@@ -11,22 +11,8 @@ FPS takes the extremes first, so a stray point is always among the first picks: 
 """
 from __future__ import annotations
 
-import numpy as np
-import torch
-
 from . import capi
-from .outliers import frame_points
-
-
-def _device() -> torch.device:
-    if not torch.cuda.is_available():
-        raise RuntimeError("farthest-point subsampling (--subsample fps) needs a CUDA GPU and libmeshanything_b200.so; "
-                           "there is no CPU fallback")
-    try:
-        capi.lib()
-    except Exception as e:
-        raise RuntimeError("farthest-point subsampling (--subsample fps) needs libmeshanything_b200.so: " + str(e)) from e
-    return torch.device("cuda", torch.cuda.current_device())
+from .pointcloud import frame_points, require_gpu
 
 
 def farthest_point_sample(points, m: int = 4096, start: int = 0):
@@ -34,8 +20,5 @@ def farthest_point_sample(points, m: int = 4096, start: int = 0):
 
     1 <= m <= N <= 2^24, 0 <= start < N.  r2[m - 1] is the squared covering radius of the whole subset in the output
     frame: every point lies within sqrt(r2[m - 1]) of a pick."""
-    dev = _device()
-    shape = tuple(points.shape) if hasattr(points, "shape") else np.shape(points)
-    if len(shape) != 2 or shape[1] != 3:
-        raise ValueError(f"farthest_point_sample: points [N, 3], got {shape}")
-    return capi.farthest_point_sample(frame_points(points, dev).contiguous(), m, start)
+    dev = require_gpu("farthest-point subsampling (--subsample fps)")
+    return capi.farthest_point_sample(frame_points(points, dev, "farthest_point_sample"), m, start)

@@ -1,6 +1,6 @@
 """-m gpu: the normal estimator of `--input_type pc` (csrc/normals.cu) against its numpy restatement
-(tests/normals_oracle.py) -- kNN indices, unoriented and oriented normals bit for bit -- exact kNN at 1M points, and the
-pipeline: `Dataset('pc')` and `main.py --input_type pc`."""
+(tests/normals_oracle.py) -- kNN indices, unoriented and oriented normals bit for bit -- exact kNN at 1M points, bad
+input refused before any launch, and the pipeline: `Dataset('pc')` and `main.py --input_type pc`."""
 import os
 import subprocess
 import sys
@@ -99,6 +99,24 @@ def test_one_million_points_exact_knn_and_outward_sphere():
     out = (nrm * sf).sum(dim=1)
     assert bool((out > 0).all()), int((out <= 0).sum())
     print(f"1M wand points: {rounds} Boruvka rounds; 1M sphere: {capi.lib().ma_estimate_normals_last_rounds()} rounds")
+
+
+@gpu
+def test_bad_input_raises_before_any_launch():
+    dev = _dev()
+    ok = torch.rand(100, 3, device=dev) - 0.5
+    L = capi.lib()
+    bad = [((ok.cpu(),), {}), ((ok.double(),), {}), ((ok[:, :2].contiguous(),), {}), ((ok.t().contiguous().t(),), {}),
+           ((ok[:16].contiguous(),), {}), ((ok.cpu().numpy(),), {}),
+           ((torch.full((100, 3), float("nan"), device=dev),), {}), ((torch.full((100, 3), float("inf"), device=dev),), {}),
+           ((ok,), {"k": 0}), ((ok,), {"k": 65}), ((ok,), {"k": 2.5}), ((ok,), {"k": True})]
+    torch.cuda.synchronize()
+    before = L.ma_launch_count()
+    for args, kw in bad:
+        with pytest.raises(ValueError):
+            capi.estimate_normals(*args, **kw)
+    assert L.ma_launch_count() == before
+    capi.estimate_normals(ok[:65].contiguous(), k=64)  # the edges of every range are accepted
 
 
 def _mouse():

@@ -13,7 +13,7 @@ import torch
 
 from meshanything_b200 import capi
 from meshanything_b200.objects import split_objects
-from meshanything_b200.outliers import frame_points
+from meshanything_b200.pointcloud import frame_points
 from tests import objects_oracle as O
 from tests import outliers_oracle as OO
 from tests import plane_oracle as P

@@ -1,6 +1,7 @@
 """-m gpu: outlier removal (csrc/outliers.cu) against its numpy restatement (tests/outliers_oracle.py) bit for bit --
 keep mask, kept indices, mean distances, mu, sigma, threshold, counts -- the exact kNN of its robust grid at 1M points
-with far outliers, and the pipeline: `Dataset(..., outliers=...)` for `pc` and `pc_normal`, `main.py --remove_outliers`."""
+with far outliers, bad input refused before any launch, and the pipeline: `Dataset(..., outliers=...)` for `pc` and
+`pc_normal`, `main.py --remove_outliers`."""
 import os
 import subprocess
 import sys
@@ -10,7 +11,8 @@ import pytest
 import torch
 
 from meshanything_b200 import capi, metrics
-from meshanything_b200.outliers import frame_points, remove_outliers
+from meshanything_b200.outliers import remove_outliers
+from meshanything_b200.pointcloud import frame_points
 from tests import outliers_oracle as O
 
 gpu = pytest.mark.gpu
@@ -122,6 +124,25 @@ def test_one_million_points_with_far_outliers_exact_knn():
     assert int(keep[n - m:].sum()) < m // 100                           # nearly every far point goes
     assert int(keep[:n - m].sum()) > 0.97 * (n - m)
     print(f"1M + 1 % far: kept {int(st[6])}, {int(st[4])} components, {int(st[7])} rounds")
+
+
+@gpu
+def test_bad_input_raises_before_any_launch():
+    dev = _dev()
+    ok = torch.rand(100, 3, device=dev) - 0.5
+    L = capi.lib()
+    bad = [((ok.cpu(),), {}), ((ok.double(),), {}), ((ok[:, :2].contiguous(),), {}), ((ok.t().contiguous().t(),), {}),
+           ((ok[:16].contiguous(),), {}), ((ok.cpu().numpy(),), {}),
+           ((torch.full((100, 3), float("nan"), device=dev),), {}), ((torch.full((100, 3), float("inf"), device=dev),), {}),
+           ((ok,), {"k": 0}), ((ok,), {"k": 65}), ((ok,), {"k": 2.5}), ((ok,), {"k": True}),
+           ((ok,), {"std_ratio": float("inf")}), ((ok,), {"min_component": -0.1})]
+    torch.cuda.synchronize()
+    before = L.ma_launch_count()
+    for args, kw in bad:
+        with pytest.raises(ValueError):
+            capi.remove_outliers(*args, **kw)
+    assert L.ma_launch_count() == before
+    capi.remove_outliers(ok[:65].contiguous(), k=64)  # the edges of every range are accepted
 
 
 def _stray_sphere(seed, n=8000, strays=20):

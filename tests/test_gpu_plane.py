@@ -11,7 +11,7 @@ import pytest
 import torch
 
 from meshanything_b200 import capi
-from meshanything_b200.outliers import frame_points
+from meshanything_b200.pointcloud import frame_points
 from meshanything_b200.plane import remove_plane
 from tests import outliers_oracle as OO
 from tests import plane_oracle as P

@@ -11,7 +11,8 @@ import pytest
 import torch
 
 from meshanything_b200 import capi
-from meshanything_b200.outliers import frame_points, remove_outliers
+from meshanything_b200.outliers import remove_outliers
+from meshanything_b200.pointcloud import frame_points
 from meshanything_b200.subsample import farthest_point_sample
 from tests import subsample_oracle as S
 

@@ -16,7 +16,6 @@ import argparse
 import ctypes as C
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -26,27 +25,12 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from bench_common import device_info, stats  # noqa: E402
 from meshanything_b200 import capi, metrics  # noqa: E402
 from meshanything_b200.inputs import synthetic_pc_normal  # noqa: E402
 
 FP32_PEAK = 67e12          # H100 SXM data sheet, dense FP32 (a card allowed up to 700 W)
 FLOP_TRI, FLOP_PT = 59, 8
-
-
-def _stats(xs):
-    xs = sorted(xs)
-    return {"median": round(xs[len(xs) // 2], 4), "min": round(xs[0], 4), "max": round(xs[-1], 4), "n": len(xs)}
-
-
-def device_info():
-    info = {"device": torch.cuda.get_device_name(0)}
-    try:
-        q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=60).stdout.strip()
-        info["power_limit"], info["max_sm_clock"] = [s.strip() for s in q.split(",")[:2]]
-    except Exception as e:  # pragma: no cover
-        info["power_limit"] = f"unavailable ({type(e).__name__})"
-    return info
 
 
 def score_workload(S, N, F, P, warmup, repeats):
@@ -75,8 +59,8 @@ def score_workload(S, N, F, P, warmup, repeats):
         ms.append(a.elapsed_time(b))
     assert torch.equal(out, terms)
     tri_pairs, pt_pairs = S * N * P * F, S * N * 16 * F * P
-    med = _stats(ms)["median"] * 1e-3
-    return {"S": S, "N": N, "F": F, "P": P, "mesh_score_ms": _stats(ms),
+    med = stats(ms)["median"] * 1e-3
+    return {"S": S, "N": N, "F": F, "P": P, "mesh_score_ms": stats(ms),
             "point_triangle_pairs": tri_pairs, "point_point_pairs": pt_pairs,
             "pair_evaluations_per_s": round((tri_pairs + pt_pairs) / med, -6),
             "kernel_share_of_fp32_datasheet_rate": round((tri_pairs * FLOP_TRI + pt_pairs * FLOP_PT) / med / FP32_PEAK, 4)}

@@ -10,10 +10,8 @@ recorded by the library between the stages, median / min / max over the repeats 
 second pair of events; the number of Boruvka rounds.  The device name and power limit are read in the same run.
 """
 import argparse
-import ctypes as C
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -22,25 +20,10 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from bench_common import device_info, stage_times  # noqa: E402
 from meshanything_b200 import capi, metrics  # noqa: E402
 
 STAGES = ("grid", "knn", "pca", "orient")
-
-
-def _stats(xs):
-    xs = sorted(xs)
-    return {"median": round(xs[len(xs) // 2], 4), "min": round(xs[0], 4), "max": round(xs[-1], 4), "n": len(xs)}
-
-
-def device_info():
-    info = {"device": torch.cuda.get_device_name(0)}
-    try:
-        q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=60).stdout.strip()
-        info["power_limit"], info["max_sm_clock"] = [s.strip() for s in q.split(",")[:2]]
-    except Exception as e:  # pragma: no cover
-        info["power_limit"] = f"unavailable ({type(e).__name__})"
-    return info
 
 
 def cloud(kind, n):
@@ -62,29 +45,16 @@ def workload(kind, n, k, warmup, repeats):
     L = capi.lib()
     ws = torch.empty(L.ma_estimate_normals_workspace_bytes(n, k), dtype=torch.uint8, device=dev)
     out = torch.empty_like(ref)
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(5)]
-    for e in ev:                                               # torch creates the CUDA event at its first record
-        e.record()
-    handles = (C.c_void_p * 5)(*[e.cuda_event for e in ev])
-    stages = {s: [] for s in STAGES}
-    total, rounds = [], set()
-    for it in range(warmup + repeats):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        L.ma_estimate_normals_set_events(handles)
-        a.record()
+    rounds = set()
+
+    def call():
         capi.check(L.ma_estimate_normals(capi.ptr(pts), n, k, capi.ptr(out), None, None, capi.ptr(ws),
                                          capi.stream_ptr()), "ma_estimate_normals")
-        b.record()
-        L.ma_estimate_normals_set_events(None)
-        b.synchronize()
         rounds.add(L.ma_estimate_normals_last_rounds())
-        if it >= warmup:
-            total.append(a.elapsed_time(b))
-            for i, s in enumerate(STAGES):
-                stages[s].append(ev[i].elapsed_time(ev[i + 1]))
+
+    times = stage_times(L.ma_estimate_normals_set_events, STAGES, call, warmup, repeats)
     assert torch.equal(out, ref)
-    return {"cloud": kind, "N": n, "k": k, "total_ms": _stats(total), **{f"{s}_ms": _stats(v) for s, v in stages.items()},
-            "boruvka_rounds": sorted(rounds)}
+    return {"cloud": kind, "N": n, "k": k, **times, "boruvka_rounds": sorted(rounds)}
 
 
 def main():

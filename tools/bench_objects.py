@@ -24,7 +24,6 @@ import argparse
 import ctypes as C
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -33,25 +32,10 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from bench_common import device_info, stage_times  # noqa: E402
 from meshanything_b200 import capi, metrics  # noqa: E402
 
 STAGES = ("grid", "connectivity", "order")
-
-
-def _stats(xs):
-    xs = sorted(xs)
-    return {"median": round(xs[len(xs) // 2], 4), "min": round(xs[0], 4), "max": round(xs[-1], 4), "n": len(xs)}
-
-
-def device_info():
-    info = {"device": torch.cuda.get_device_name(0)}
-    try:
-        q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=60).stdout.strip()
-        info["power_limit"], info["max_sm_clock"] = [s.strip() for s in q.split(",")[:2]]
-    except Exception as e:  # pragma: no cover
-        info["power_limit"] = f"unavailable ({type(e).__name__})"
-    return info
 
 
 def scene(n):
@@ -148,28 +132,14 @@ def workload(name, pts, e, warmup, repeats, brute):
     idx = torch.empty((n,), dtype=torch.int64, device=dev)
     off = torch.empty((n // mp + 1,), dtype=torch.int64, device=dev)
     st = torch.empty((6,), dtype=torch.int64, device=dev)
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
-    for x in ev:                                               # torch creates the CUDA event at its first record
-        x.record()
-    handles = (C.c_void_p * 4)(*[x.cuda_event for x in ev])
-    stages = {s: [] for s in STAGES}
-    total = []
-    for it in range(warmup + repeats):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        L.ma_split_objects_set_events(handles)
-        a.record()
+
+    def call():
         capi.check(L.ma_split_objects(capi.ptr(pts), n, C.c_float(np.float32(e)), mp, capi.ptr(lab), capi.ptr(idx),
                                       capi.ptr(off), capi.ptr(st), capi.ptr(ws), capi.stream_ptr()), "ma_split_objects")
-        b.record()
-        L.ma_split_objects_set_events(None)
-        b.synchronize()
-        if it >= warmup:
-            total.append(a.elapsed_time(b))
-            for i, s in enumerate(STAGES):
-                stages[s].append(ev[i].elapsed_time(ev[i + 1]))
+
+    times = stage_times(L.ma_split_objects_set_events, STAGES, call, warmup, repeats)
     assert torch.equal(lab, ref_lab) and torch.equal(st.cpu(), torch.from_numpy(ref_st))
-    out = {"workload": name, "N": n, "e": e, "total_ms": _stats(total),
-           **{f"{s}_ms": _stats(v) for s, v in stages.items()}, "clusters": int(ref_st[0]), "objects": int(ref_st[1]),
+    out = {"workload": name, "N": n, "e": e, **times, "clusters": int(ref_st[0]), "objects": int(ref_st[1]),
            "object_sizes": np.diff(ref_off.cpu().numpy()).tolist(), "dropped_points": int(ref_st[4])}
     if brute:
         torch_components(pts[:4096], e)                        # warm-up

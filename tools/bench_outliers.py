@@ -16,7 +16,6 @@ import argparse
 import ctypes as C
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -25,25 +24,10 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from bench_common import device_info, stage_times  # noqa: E402
 from meshanything_b200 import capi, metrics  # noqa: E402
 
 STAGES = ("grid", "knn", "stats", "components")
-
-
-def _stats(xs):
-    xs = sorted(xs)
-    return {"median": round(xs[len(xs) // 2], 4), "min": round(xs[0], 4), "max": round(xs[-1], 4), "n": len(xs)}
-
-
-def device_info():
-    info = {"device": torch.cuda.get_device_name(0)}
-    try:
-        q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=60).stdout.strip()
-        info["power_limit"], info["max_sm_clock"] = [s.strip() for s in q.split(",")[:2]]
-    except Exception as e:  # pragma: no cover
-        info["power_limit"] = f"unavailable ({type(e).__name__})"
-    return info
 
 
 def cloud(kind, n):
@@ -76,28 +60,16 @@ def workload(kind, n, k, warmup, repeats):
     idx = torch.empty((n,), dtype=torch.int64, device=dev)
     nk = torch.empty((1,), dtype=torch.int64, device=dev)
     st = torch.empty((8,), dtype=torch.float64, device=dev)
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(5)]
-    for e in ev:                                               # torch creates the CUDA event at its first record
-        e.record()
-    handles = (C.c_void_p * 5)(*[e.cuda_event for e in ev])
-    stages = {s: [] for s in STAGES}
-    total = []
-    for it in range(warmup + repeats):
-        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        L.ma_remove_outliers_set_events(handles)
-        a.record()
+
+    def call():
         capi.check(L.ma_remove_outliers(capi.ptr(pts), n, k, C.c_double(2.0), C.c_double(0.01), capi.ptr(keep),
                                         capi.ptr(idx), capi.ptr(nk), None, None, capi.ptr(st), capi.ptr(ws),
                                         capi.stream_ptr()), "ma_remove_outliers")
-        b.record()
-        L.ma_remove_outliers_set_events(None)
-        b.synchronize()
-        if it >= warmup:
-            total.append(a.elapsed_time(b))
-            for i, s in enumerate(STAGES):
-                stages[s].append(ev[i].elapsed_time(ev[i + 1]))
-    assert torch.equal(keep.bool(), ref_keep) and torch.equal(st.cpu(), torch.from_numpy(ref_st))
-    return {"cloud": kind, "N": n, "k": k, "total_ms": _stats(total), **{f"{s}_ms": _stats(v) for s, v in stages.items()},
+
+    times = stage_times(L.ma_remove_outliers_set_events, STAGES, call, warmup, repeats)
+    # every stat but the last: the number of connectivity rounds depends on the schedule of the hooking atomics
+    assert torch.equal(keep.bool(), ref_keep) and torch.equal(st.cpu()[:7], torch.from_numpy(ref_st[:7]))
+    return {"cloud": kind, "N": n, "k": k, **times,
             "kept": int(ref_st[6]), "components": int(ref_st[4]), "components_dropped": int(ref_st[5]),
             "rounds": int(ref_st[7])}
 

@@ -15,7 +15,6 @@ import argparse
 import ctypes as C
 import json
 import os
-import subprocess
 import sys
 
 import numpy as np
@@ -24,28 +23,12 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from bench_common import device_info, stats  # noqa: E402
 from meshanything_b200 import capi, metrics  # noqa: E402
 from tests.subsample_oracle import torch_bruteforce  # noqa: E402
 
 M = 4096
 PATHS = {1: "one_cta", 2: "grid_shared", 3: "grid_global"}
-
-
-def _stats(xs):
-    xs = sorted(xs)
-    return {"median": round(xs[len(xs) // 2], 4), "min": round(xs[0], 4), "max": round(xs[-1], 4), "n": len(xs)}
-
-
-def device_info():
-    info = {"device": torch.cuda.get_device_name(0),
-            "sms": torch.cuda.get_device_properties(0).multi_processor_count}
-    try:
-        q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=60).stdout.strip()
-        info["power_limit"], info["max_sm_clock"] = [s.strip() for s in q.split(",")[:2]]
-    except Exception as e:  # pragma: no cover
-        info["power_limit"] = f"unavailable ({type(e).__name__})"
-    return info
 
 
 def wand(n):
@@ -66,7 +49,7 @@ def _time(fn, warmup, repeats):
         b.synchronize()
         if it >= warmup:
             times.append(a.elapsed_time(b))
-    return out, _stats(times)
+    return out, stats(times)
 
 
 def workload(n, warmup, repeats):
@@ -117,7 +100,8 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("bench_subsample: needs a CUDA device")
     runs = [workload(n, args.warmup, args.repeats) for n in (8192, 12_288, 100_000, 1_000_000, 4_000_000)]
-    result = {"bench": "subsample", **device_info(), "runs": runs}
+    result = {"bench": "subsample", **device_info(), "sms": torch.cuda.get_device_properties(0).multi_processor_count,
+              "runs": runs}
     line = json.dumps(result)
     print(line)
     if args.out:

@@ -12,7 +12,6 @@ oracle's host time on the wand at n = 128, for context, and the device name and 
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -22,6 +21,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+from bench_common import device_info, stats  # noqa: E402
 import mesh_to_pc  # noqa: E402
 from meshanything_b200 import capi  # noqa: E402
 
@@ -53,11 +53,6 @@ def icosphere_soup(m=224, seed=0):
     noise = sum(np.sin(k[q, 0] * v[:, 0] + ph[q, 0]) * np.sin(k[q, 1] * v[:, 1] + ph[q, 1])
                 * np.sin(k[q, 2] * v[:, 2] + ph[q, 2]) for q in range(3))
     return v * (0.8 * (1 + 0.03 * noise))[:, None], np.concatenate(faces)
-
-
-def _stats(xs):
-    xs = sorted(xs)
-    return {"median": round(xs[len(xs) // 2], 4), "min": round(xs[0], 4), "max": round(xs[-1], 4), "n": len(xs)}
 
 
 def _events(fn, warmup, repeats):
@@ -93,20 +88,9 @@ def run(name, vertices, faces, n, warmup, repeats):
         torch.cuda.synchronize()
         if i >= warmup:
             e2e.append((time.perf_counter() - t0) * 1e3)
-    return {"workload": name, "n": n, "input_faces": int(len(faces)), "udf_ms": _stats(udf_ms),
-            "marching_cubes_ms": _stats(mc_ms), "export_to_watertight_ms": _stats(e2e),
+    return {"workload": name, "n": n, "input_faces": int(len(faces)), "udf_ms": stats(udf_ms),
+            "marching_cubes_ms": stats(mc_ms), "export_to_watertight_ms": stats(e2e),
             "out_vertices": int(mv.shape[0]), "out_faces": int(mf.shape[0])}
-
-
-def device_info():
-    info = {"device": torch.cuda.get_device_name(0)}
-    try:
-        q = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader"],
-                           capture_output=True, text=True, timeout=60).stdout.strip()
-        info["power_limit"], info["max_sm_clock"] = [s.strip() for s in q.split(",")[:2]]
-    except Exception as e:  # pragma: no cover
-        info["power_limit"] = f"unavailable ({type(e).__name__})"
-    return info
 
 
 def main():
