@@ -447,6 +447,27 @@ int ma_split_objects(const float* xyz, int n, float e, int min_points, int32_t* 
  * sizes) and the order and selection (NULL: off). */
 void ma_split_objects_set_events(void* const* events);
 
+/* ---- moving-least-squares smoothing of a point cloud (`--smooth`; csrc/smooth.cu) --------------------------------
+ * xyz fp32 [n][3], finite, already in the output frame -> out_xyz fp32 [n][3], every point projected onto the weighted
+ * quadratic height field fitted to it and its k nearest other points, as DESIGN.md section 1.8 defines it: weights
+ * (1 - d^2 / H)^2 with H = 2 d^2 of the k-th neighbour (fp64 d^2), the weighted centroid and covariance, the local frame
+ * from 5 cyclic Jacobi sweeps, z = a . (1, u, v, u^2, uv, v^2) over (u, v) scaled by sqrt(H), solved by Cholesky.
+ * A Cholesky pivot at or below 1e-9 sum w (the singular fallback) or a move by more than sqrt(H) (the
+ * far fallback) projects the point onto the weighted plane instead.  stats_out int64 [3] (device) = (quadratic fits,
+ * singular fallbacks, far fallbacks).  Optional test outputs (NULL: not written): normal_out fp32 [n][3] (the unit
+ * normal of each local frame, unoriented), flag_out uint8 [n] (0 quadratic, 1 singular, 2 far), knn_out int32 [n][k]
+ * (rank order).  5 <= k <= 64, k < n <= 2^24.  ws: ma_smooth_points_workspace_bytes(n, k) bytes (needs the device: it
+ * sizes CUB's scan; 0 for shapes out of range).  No host synchronisation and no floating-point atomics: two calls give
+ * identical bits. */
+size_t ma_smooth_points_workspace_bytes(int n, int k);
+int ma_smooth_points(const float* xyz, int n, int k, float* out_xyz, float* normal_out, uint8_t* flag_out,
+                     int32_t* knn_out, int64_t* stats_out, void* ws, void* stream);
+/* Measurement hooks (tools/bench_smooth.py): events = 4 cudaEvent_t recorded on the stream of every following call at
+ * its start and after the grid build, the kNN and the fit (NULL: off); the order the fit threads walk the points in
+ * (1, the default: cell order; 0: index order).  Neither changes a result. */
+void ma_smooth_points_set_events(void* const* events);
+void ma_smooth_points_set_order(int cell_order);
+
 /* number of kernels launched by the library since load (bench.py's gpu_launches) */
 unsigned long long ma_launch_count(void);
 

@@ -5,6 +5,7 @@
     python main.py --input_type pc --input_path scan.npy --remove_outliers   # drop stray points / floaters first
     python main.py --input_type pc --input_path scan.npy --subsample fps     # even coverage of uneven scan density
     python main.py --input_type pc --input_path scan.npy --remove_plane      # drop the table / floor under the object
+    python main.py --input_type pc --input_path scan.npy --smooth            # pull scanner noise back onto the surface
     python main.py --input_type pc --input_path scan.npy --remove_plane --split_objects --output_frame input
                                                    # one mesh per object on the table, each where it stands in the scan
     torchrun --nproc-per-node 8 main.py --input_type pc_normal --input_dir pcs --batchsize_per_gpu 64
@@ -60,6 +61,18 @@ def _remove_plane(xyz, path, plane, n_points=4096):
     return idx.cpu().numpy()
 
 
+def _smooth(xyz, path, smooth):
+    """`--smooth`: xyz [N, 3] projected onto the moving-least-squares surface of DESIGN.md section 1.8 (on the GPU,
+    meshanything_b200.smooth), in xyz's dtype and units; every row is kept and nothing is drawn.  One line per input
+    with the counts and the displacements in input units."""
+    from meshanything_b200.smooth import smooth_points
+    out, st = smooth_points(xyz, **smooth)
+    print(f"{_uid_of(path)}: smoothed {st.n_points} points (k = {st.k}): {st.quadratic} on their quadratic, "
+          f"{st.singular} singular and {st.far} far onto their plane; moved {st.mean_displacement:.4g} on average, "
+          f"{st.max_displacement:.4g} at most (input units)")
+    return out.cpu().numpy()
+
+
 def _split_objects(xyz, path, objects, n_points=4096):
     """`--split_objects`: the point indices of every object of xyz [N, 3] that DESIGN.md section 1.7 defines (on the
     GPU, meshanything_b200.objects), objects in order, each ascending; one line per input with the clusters, the
@@ -88,12 +101,13 @@ def _farthest_points(xyz, path, n_points=4096):
     return idx.cpu().numpy()
 
 
-def _subsample_points(path, n_points=4096, outliers=None, subsample='random', plane=None, objects=None):
+def _subsample_points(path, n_points=4096, outliers=None, subsample='random', plane=None, objects=None, smooth=None):
     """`--input_type pc_normal`: an .npy of >= 4096 (xyz, normal) rows; a random 4096-subset without replacement
     (global numpy RNG, seeded by --seed as the reference does through accelerate.set_seed), or with
     subsample='fps' the farthest-point subset of the xyz columns.  With `outliers` (the keyword arguments of
     meshanything_b200.outliers.remove_outliers) the rows are first cleaned by their xyz; with `plane` (the keyword
-    arguments of meshanything_b200.plane.remove_plane) the support plane goes before that.  With `objects` ({'distance':
+    arguments of meshanything_b200.plane.remove_plane) the support plane goes before that.  With `smooth` ({'k': k})
+    the xyz columns of the cleaned rows are smoothed; the normals pass through unchanged.  With `objects` ({'distance':
     e}) the cleaned cloud is split into objects and a list of one subset per object is returned, drawn in object
     order."""
     cloud = np.load(path)
@@ -101,6 +115,9 @@ def _subsample_points(path, n_points=4096, outliers=None, subsample='random', pl
         cloud = cloud[_remove_plane(cloud[:, :3], path, plane, n_points)]
     if outliers is not None:
         cloud = cloud[_remove_outliers(cloud[:, :3], path, outliers, n_points)]
+    if smooth is not None:
+        cloud = cloud.copy()
+        cloud[:, :3] = _smooth(cloud[:, :3], path, smooth)
     assert cloud.shape[0] >= n_points, "input pc_normal should have at least 4096 points"
     if objects is not None:
         return [_subset(cloud[part], path, n_points, subsample)
@@ -116,14 +133,16 @@ def _subset(cloud, path, n_points, subsample):
     return cloud[keep]
 
 
-def _points_with_normals(path, n_points=4096, k=16, outliers=None, subsample='random', plane=None, objects=None):
+def _points_with_normals(path, n_points=4096, k=16, outliers=None, subsample='random', plane=None, objects=None,
+                         smooth=None):
     """`--input_type pc`: a bare cloud (.npy (N, 3) or vertex-only .ply) of >= 4096 points.  Normals are estimated on
     the GPU from all N points (meshanything_b200.normals), then the same 4096-subset as `pc_normal` is drawn: the
     xyz-only copy of a file selects the points the file with normals selects under the same seed.  With `outliers`
     the cloud is cleaned first, and normals and subset come from the kept points; `plane` removes the support plane
-    before that.  With `objects` the cleaned cloud is split into objects first, and every object gets its own normals
-    (estimated on its points alone, so that their orientation is rooted at its own farthest point) and subset, in
-    object order: a list of one cloud per object is returned."""
+    before that; `smooth` smooths the cleaned points before their normals are estimated.  With `objects` the cleaned
+    cloud is split into objects first, and every object gets its own normals (estimated on its points alone, so that
+    their orientation is rooted at its own farthest point) and subset, in object order: a list of one cloud per object
+    is returned."""
     from mesh_to_pc import load_points
     xyz = load_points(path)
     if not np.issubdtype(xyz.dtype, np.floating):
@@ -133,6 +152,8 @@ def _points_with_normals(path, n_points=4096, k=16, outliers=None, subsample='ra
         xyz = xyz[_remove_plane(xyz, path, plane, n_points)]
     if outliers is not None:
         xyz = xyz[_remove_outliers(xyz, path, outliers, n_points)]
+    if smooth is not None:
+        xyz = _smooth(xyz, path, smooth)
     if objects is not None:
         return [_with_normals(xyz[part], path, n_points, k, subsample)
                 for part in _split_objects(xyz, path, objects, n_points)]
@@ -160,6 +181,8 @@ _NO_MESH_FPS = ("--subsample fps applies to point-cloud input (--input_type pc o
                 "already sampled uniformly by area")
 _NO_MESH_OBJECTS = ("--split_objects applies to point-cloud input (--input_type pc or pc_normal): splitting a mesh into "
                     "its connected parts is not supported")
+_NO_MESH_SMOOTH = ("--smooth applies to point-cloud input (--input_type pc or pc_normal): the points of a mesh are "
+                   "sampled exactly from its surface and carry no scanner noise")
 _NO_MESH_PLANE = ("--remove_plane applies to point-cloud input (--input_type pc or pc_normal): the points of a mesh are "
                   "sampled from its own surface, which has no scanned support under it")
 SUBSAMPLERS = ('random', 'fps')
@@ -181,19 +204,26 @@ class Dataset:
     (farthest-point sampling on the GPU, DESIGN.md section 1.4).  `plane` (point clouds only): None, or the keyword
     arguments of meshanything_b200.plane.remove_plane, to remove the support plane (a table, the floor) first.
     `objects` (point clouds only): None, or {'distance': e}, to split every cloud after plane and outlier removal into
-    objects (DESIGN.md section 1.7), each its own item with uid `{uid}_obj{k}`.  Items also carry 'frame', the
+    objects (DESIGN.md section 1.7), each its own item with uid `{uid}_obj{k}`.  `smooth` (point clouds only): None, or
+    {'k': k}, to smooth every cloud after plane and outlier removal (DESIGN.md section 1.8; for pc_normal only the xyz
+    columns move).  Items also carry 'frame', the
     metrics.shape_frame of the rows before normalisation, which metrics.to_input_frame applies to put a mesh back in
     the input's coordinates."""
 
-    def __init__(self, input_type, input_list, mc=False, outliers=None, subsample='random', plane=None, objects=None):
+    def __init__(self, input_type, input_list, mc=False, outliers=None, subsample='random', plane=None, objects=None,
+                 smooth=None):
         if outliers is not None and input_type not in ('pc', 'pc_normal'):
             raise ValueError(_NO_MESH_OUTLIERS)
         if plane is not None and input_type not in ('pc', 'pc_normal'):
             raise ValueError(_NO_MESH_PLANE)
         if objects is not None and input_type not in ('pc', 'pc_normal'):
             raise ValueError(_NO_MESH_OBJECTS)
+        if smooth is not None and input_type not in ('pc', 'pc_normal'):
+            raise ValueError(_NO_MESH_SMOOTH)
         _check_subsample(input_type, subsample)
         kw = dict(outliers=outliers, subsample=subsample, plane=plane, objects=objects)
+        if smooth is not None:
+            kw['smooth'] = smooth
         if input_type == 'pc_normal':
             clouds = [_subsample_points(p, **kw) for p in input_list]
         elif input_type == 'pc':
@@ -264,6 +294,15 @@ def get_args():
     # box's longest side; DESIGN.md section 1.7; meshanything_b200.objects) and mesh each one on its own
     parser.add_argument('--split_objects', default=False, action="store_true")
     parser.add_argument('--object_distance', default=0.02, type=float)
+    # not in the reference: pull scanner noise back onto the surface by projecting every point onto the quadratic
+    # fitted to its --smooth_neighbors nearest points (moving least squares on the GPU; DESIGN.md section 1.8;
+    # meshanything_b200.smooth), after plane and outlier removal and before normals and the subset; for pc_normal input
+    # only the xyz columns move, the file's normals pass through unchanged
+    parser.add_argument('--smooth', default=False, action="store_true",
+                        help="smooth scanner noise by moving-least-squares projection (point-cloud input; for "
+                             "pc_normal only xyz moves, the normals pass through unchanged)")
+    parser.add_argument('--smooth_neighbors', default=24, type=int,
+                        help="neighbours of each point's local fit for --smooth, 5..64 (default 24)")
     # not in the reference: write meshes in the model's [-0.5, 0.5) frame (model, the reference's output) or back in
     # the input's coordinates (input: c + L v with the bounding box centre c and longest side L of the shape's points)
     parser.add_argument('--output_frame', default='model', choices=OUTPUT_FRAMES)
@@ -290,6 +329,13 @@ def object_options(args):
     if not getattr(args, 'split_objects', False):
         return None
     return {'distance': getattr(args, 'object_distance', 0.02)}
+
+
+def smooth_options(args):
+    """The `smooth` argument of Dataset from the command line: None without --smooth."""
+    if not getattr(args, 'smooth', False):
+        return None
+    return {'k': getattr(args, 'smooth_neighbors', 24)}
 
 
 def check_args(args):
@@ -326,6 +372,12 @@ def check_args(args):
         if not (np.isfinite(distance) and 0 < distance <= 1 and np.float32(distance) * np.float32(distance) > 0):
             raise ValueError(f"--object_distance must be in (0, 1] (a share of the bounding box's longest side, with a "
                              f"square above 0 in fp32), got {distance}")
+    if getattr(args, 'smooth', False):
+        if args.input_type == 'mesh':
+            raise ValueError(_NO_MESH_SMOOTH)
+        k = getattr(args, 'smooth_neighbors', 24)
+        if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 5 <= k <= 64:
+            raise ValueError(f"--smooth_neighbors must be in 5..64, got {k}")
     if getattr(args, 'output_frame', 'model') not in OUTPUT_FRAMES:
         raise ValueError(f"--output_frame must be one of {', '.join(OUTPUT_FRAMES)}, got {args.output_frame!r}")
 
@@ -452,7 +504,7 @@ if __name__ == "__main__":
     np.random.seed(args.seed)
     torch.manual_seed(args.seed)
     dataset = Dataset(args.input_type, input_list, args.mc, outliers=outlier_options(args), subsample=args.subsample,
-                      plane=plane_options(args), objects=object_options(args))
+                      plane=plane_options(args), objects=object_options(args), smooth=smooth_options(args))
 
     bs = args.batchsize_per_gpu
     batches = [list(range(i, min(i + bs, len(dataset)))) for i in range(0, len(dataset), bs)]

@@ -55,6 +55,7 @@ EXPORTS = [
     "ma_farthest_point_sample_last_path",
     "ma_remove_plane_workspace_bytes", "ma_remove_plane", "ma_remove_plane_set_events",
     "ma_split_objects_workspace_bytes", "ma_split_objects", "ma_split_objects_set_events",
+    "ma_smooth_points_workspace_bytes", "ma_smooth_points", "ma_smooth_points_set_events", "ma_smooth_points_set_order",
     "ma_fourier_embed_f16", "ma_scatter_heads_f16", "ma_residual_add", "ma_convert_rows", "ma_add_table",
     "ma_gather_codes", "ma_coords",
 ]
@@ -162,6 +163,13 @@ def lib():
     L.ma_split_objects.argtypes = [_vp, C.c_int, C.c_float, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp]
     L.ma_split_objects_set_events.argtypes = [_vp]
     L.ma_split_objects_set_events.restype = None
+    L.ma_smooth_points_workspace_bytes.argtypes = [C.c_int, C.c_int]
+    L.ma_smooth_points_workspace_bytes.restype = C.c_size_t
+    L.ma_smooth_points.argtypes = [_vp, C.c_int, C.c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp]
+    L.ma_smooth_points_set_events.argtypes = [_vp]
+    L.ma_smooth_points_set_events.restype = None
+    L.ma_smooth_points_set_order.argtypes = [C.c_int]
+    L.ma_smooth_points_set_order.restype = None
     L.ma_fourier_embed_f16.argtypes = [_vp, C.c_long, _vp, _vp]
     L.ma_scatter_heads_f16.argtypes = [_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_long, _vp, C.c_long, _vp]
     L.ma_residual_add.argtypes = [_vp, _vp, _vp, C.c_long, _vp]
@@ -594,6 +602,34 @@ def split_objects(points: torch.Tensor, distance: float = 0.02, min_points: int 
                                      ptr(stats), ptr(ws), stream_ptr()), "ma_split_objects")
         st = stats.cpu().numpy()
     return labels, idx[:int(st[2])], offsets[:int(st[1]) + 1], st
+
+
+SMOOTH_MIN_K = 5
+
+
+def smooth_points(points: torch.Tensor, k: int = 24, want_terms: bool = False):
+    """Moving-least-squares smoothing of a cloud (ma_smooth_points; smooth.smooth_points adds the frame map and the way
+    back to the input's units).
+
+    points fp32 [N, 3], contiguous, on a CUDA device, finite, already in the output frame; 5 <= k <= 64,
+    k < N <= 2^24.  Returns (smoothed points fp32 [N, 3] in the frame, stats int64 [3] on the host: quadratic fits,
+    singular fallbacks, far fallbacks); with want_terms also (unit normal of every local frame fp32 [N, 3], outcome
+    uint8 [N]: 0 quadratic, 1 singular, 2 far, kNN int32 [N, k] in rank order).  Every bad input raises ValueError
+    before anything is launched.  Reads the stats back (synchronises)."""
+    k = _check_int("smooth_points", "k", k, SMOOTH_MIN_K, 64)
+    n = _check_points("smooth_points", points, k + 1)
+    dev = points.device
+    ws = torch.empty(lib().ma_smooth_points_workspace_bytes(n, k), dtype=torch.uint8, device=dev)
+    out = torch.empty((n, 3), dtype=torch.float32, device=dev)
+    stats = torch.empty((3,), dtype=torch.int64, device=dev)
+    normals = torch.empty((n, 3), dtype=torch.float32, device=dev) if want_terms else None
+    flags = torch.empty((n,), dtype=torch.uint8, device=dev) if want_terms else None
+    knn = torch.empty((n, k), dtype=torch.int32, device=dev) if want_terms else None
+    with torch.cuda.device(dev):
+        check(lib().ma_smooth_points(ptr(points), n, k, ptr(out), ptr(normals), ptr(flags), ptr(knn), ptr(stats),
+                                     ptr(ws), stream_ptr()), "ma_smooth_points")
+        st = stats.cpu().numpy()
+    return (out, st, normals, flags, knn) if want_terms else (out, st)
 
 
 def tensor_core_linear_counts():

@@ -1,6 +1,6 @@
-// jacobi3.cuh -- the eigenvector of the smallest eigenvalue of a symmetric 3x3 matrix by a fixed cyclic Jacobi
-// (DESIGN.md section 1.2), shared by the per-point PCA of normals.cu and the plane refit of plane.cu.  Every fp64 step
-// is an explicit round-to-nearest intrinsic (nvcc contracts fp64 as well), so tests/normals_oracle.py (jacobi,
+// jacobi3.cuh -- eigenvectors of a symmetric 3x3 matrix by a fixed cyclic Jacobi (DESIGN.md section 1.2), shared by
+// the per-point PCA of normals.cu, the plane refit of plane.cu and the local frame of smooth.cu.  Every fp64 step is an
+// explicit round-to-nearest intrinsic (nvcc contracts fp64 as well), so tests/normals_oracle.py (jacobi,
 // smallest_vector) restates it bit for bit.
 #pragma once
 
@@ -8,11 +8,14 @@ namespace ma {
 
 constexpr int kJacobiSweeps = 5;   // cyclic sweeps: 4 reach 4e-15 rad against LAPACK on separated spectra, 1 spare
 
-// c = (xx, xy, xz, yy, yz, zz) -> v: after kJacobiSweeps sweeps over the pairs (0,1), (0,2), (1,2), the column of V of
-// the smallest diagonal entry (the lowest column on ties), divided by its fp64 length
-__device__ __forceinline__ void jacobi3_smallest(const double c[6], double v[3]) {
+// c = (xx, xy, xz, yy, yz, zz) -> the diagonal d and V (eigenvectors in its columns) after kJacobiSweeps sweeps over
+// the pairs (0,1), (0,2), (1,2)
+__device__ __forceinline__ void jacobi3(const double c[6], double d[3], double V[3][3]) {
   double A[3][3] = {{c[0], c[1], c[2]}, {c[1], c[3], c[4]}, {c[2], c[4], c[5]}};
-  double V[3][3] = {{1.0, 0.0, 0.0}, {0.0, 1.0, 0.0}, {0.0, 0.0, 1.0}};
+#pragma unroll
+  for (int a = 0; a < 3; a++)
+#pragma unroll
+    for (int b = 0; b < 3; b++) V[a][b] = a == b ? 1.0 : 0.0;
   for (int sweep = 0; sweep < kJacobiSweeps; sweep++) {
 #pragma unroll
     for (int pr = 0; pr < 3; pr++) {
@@ -40,14 +43,36 @@ __device__ __forceinline__ void jacobi3_smallest(const double c[6], double v[3])
       }
     }
   }
-  // the column of the smallest diagonal entry, the lowest column on ties
-  double v0 = V[0][0], v1 = V[1][0], v2 = V[2][0], dmin = A[0][0];
-  if (A[1][1] < dmin) { v0 = V[0][1]; v1 = V[1][1]; v2 = V[2][1]; dmin = A[1][1]; }
-  if (A[2][2] < dmin) { v0 = V[0][2]; v1 = V[1][2]; v2 = V[2][2]; }
-  const double ln = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(v0, v0), __dmul_rn(v1, v1)), __dmul_rn(v2, v2)));
-  v[0] = __ddiv_rn(v0, ln);
-  v[1] = __ddiv_rn(v1, ln);
-  v[2] = __ddiv_rn(v2, ln);
+  d[0] = A[0][0];
+  d[1] = A[1][1];
+  d[2] = A[2][2];
+}
+
+// the column of V of the smallest diagonal entry (the lowest column on ties)
+__device__ __forceinline__ int jacobi3_smallest_column(const double d[3]) {
+  int m = 0;
+  double dmin = d[0];
+  if (d[1] < dmin) { m = 1; dmin = d[1]; }
+  if (d[2] < dmin) m = 2;
+  return m;
+}
+
+// (x, y, z) divided by its fp64 length
+__device__ __forceinline__ void jacobi3_unit(double x, double y, double z, double v[3]) {
+  const double ln = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)), __dmul_rn(z, z)));
+  v[0] = __ddiv_rn(x, ln);
+  v[1] = __ddiv_rn(y, ln);
+  v[2] = __ddiv_rn(z, ln);
+}
+
+// c -> v: the column of V of the smallest diagonal entry (the lowest column on ties), divided by its fp64 length
+__device__ __forceinline__ void jacobi3_smallest(const double c[6], double v[3]) {
+  double d[3], V[3][3];
+  jacobi3(c, d, V);
+  double v0 = V[0][0], v1 = V[1][0], v2 = V[2][0], dmin = d[0];
+  if (d[1] < dmin) { v0 = V[0][1]; v1 = V[1][1]; v2 = V[2][1]; dmin = d[1]; }
+  if (d[2] < dmin) { v0 = V[0][2]; v1 = V[1][2]; v2 = V[2][2]; }
+  jacobi3_unit(v0, v1, v2, v);
 }
 
 }  // namespace ma

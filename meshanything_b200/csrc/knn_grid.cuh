@@ -1,4 +1,5 @@
-// knn_grid.cuh -- the exact kNN of DESIGN.md section 1.2 on a uniform grid, shared by normals.cu and outliers.cu.
+// knn_grid.cuh -- the exact kNN of DESIGN.md section 1.2 on a uniform grid, shared by normals.cu, outliers.cu and
+// smooth.cu.
 //
 //   grid   knn_cell_kernel counts the points per cell of a G^3 grid of cubic cells (origin lo, `scale` cells per unit;
 //          points outside are clamped into the border cells), a CUB exclusive scan gives the cell starts,
@@ -37,6 +38,12 @@ struct KnnGrid {
 static inline int knn_grid_size(int n, int k) {
   const int g = (int)ceil(0.5 * sqrt((double)n / (double)k));
   return g < 1 ? 1 : (g > kKnnMaxG ? kKnnMaxG : g);
+}
+
+// the grid over the whole output frame [-0.5, 0.5]^3 (normals.cu, smooth.cu)
+static inline KnnGrid knn_frame_grid(int n, int k) {
+  const int G = knn_grid_size(n, k);
+  return KnnGrid{{-0.5f, -0.5f, -0.5f}, (float)G, 1.0f / (float)G, G};
 }
 
 __device__ __forceinline__ int knn_cell1(float x, float lo, float scale, int G) {

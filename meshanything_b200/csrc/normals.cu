@@ -30,12 +30,6 @@ constexpr int kNmThreads = 256;
 constexpr int kNmMaxN = 1 << 24;    // vertex words hold the root in 31 bits; the index part of a kNN key in 32
 constexpr int kNmMaxRounds = 64;    // Boruvka at least halves the components with an outgoing edge per round
 
-// the grid over the whole frame [-0.5, 0.5]^3
-static KnnGrid nm_grid(int n, int k) {
-  const int G = knn_grid_size(n, k);
-  return KnnGrid{{-0.5f, -0.5f, -0.5f}, (float)G, 1.0f / (float)G, G};
-}
-
 __device__ __forceinline__ float nm_dot(float ax, float ay, float az, float bx, float by, float bz) {
   return __fadd_rn(__fadd_rn(__fmul_rn(ax, bx), __fmul_rn(ay, by)), __fmul_rn(az, bz));
 }
@@ -229,7 +223,7 @@ struct NmBuffers {
 };
 
 static NmBuffers nm_buffers(int n, int k, void* ws) {
-  const int G = nm_grid(n, k).G;
+  const int G = knn_frame_grid(n, k).G;
   const size_t cells = (size_t)G * G * G, nk = (size_t)n * k;
   Carver c(ws);
   NmBuffers b;
@@ -280,7 +274,7 @@ int ma_estimate_normals(const float* xyz, int n, int k, float* normals_out, int3
   NmBuffers b = nm_buffers(n, k, ws);
   if (knn_out) b.knn = knn_out;
   if (unoriented_out) b.uno = unoriented_out;
-  const KnnGrid grid = nm_grid(n, k);
+  const KnnGrid grid = knn_frame_grid(n, k);
   const size_t nk = (size_t)n * k;
 
   nm_events.mark(0, st);
