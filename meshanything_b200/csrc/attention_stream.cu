@@ -144,7 +144,12 @@ __global__ void __launch_bounds__(AS_THREADS, 2) attention_stream_kernel(AttnStr
           if (u >= SLOTS) mbar_wait(&sm.empty[s], ((u / SLOTS) & 1) ^ 1);
           if (old > 0) {
             mbar_expect_tx(&sm.full[s], (uint32_t)old * HD * 2);
-            bulk_g2s(sm.ring[s], (kv ? a.V : a.K) + base, (uint32_t)old * HD * 2, &sm.full[s]);
+            // a single row (the batch-1 step) reads each cache row once per step: evict_first keeps the up to 30 MB of a
+            // layer's cache from pushing the step's other data out of L2
+            if (SLOTS == AS_SLOTS_ROW)
+              bulk_g2s_evict_first(sm.ring[s], (kv ? a.V : a.K) + base, (uint32_t)old * HD * 2, &sm.full[s]);
+            else
+              bulk_g2s(sm.ring[s], (kv ? a.V : a.K) + base, (uint32_t)old * HD * 2, &sm.full[s]);
           } else {
             mbar_arrive(&sm.full[s]);   // only the current token in this chunk: nothing to load
           }

@@ -177,6 +177,18 @@ __device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t by
                "l"(src), "r"(bytes), "r"(smem_u32(bar))
                : "memory");
 }
+// The same copy with the L2 evict_first policy: for bytes read once per step (the batch-1 weight slabs and KV rows), so
+// that their lines are the first to go and the small data the step reuses (activations, residual stream, partials)
+// stays in L2
+__device__ __forceinline__ void bulk_g2s_evict_first(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
+  uint64_t pol;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
+  asm volatile(
+      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;" ::"r"(
+          smem_u32(dst)),
+      "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(pol)
+      : "memory");
+}
 
 // ---- programmatic dependent launch -----------------------------------------------------------
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }

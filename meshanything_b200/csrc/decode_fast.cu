@@ -8,6 +8,9 @@
 //   * that prefetch is issued BEFORE griddepcontrol.wait: with PDL the CTAs of kernel k+1 (and k+2..)
 //     are already resident and streaming their weights while kernel k is still computing, so HBM
 //     never idles across the 121 dependent phases of a token;
+//   * each weight byte is read once per token, so the slab copies (and the attention's KV rows) carry the L2 evict_first
+//     policy: 621 MB of weights and up to 30 MB of KV per layer stream through L2 without displacing the small data
+//     that the next kernels read back (activations, residual stream, attention partials, the argmax candidates);
 //   * activations never leave L2: residual add + LayerNorm are recomputed by every CTA in its
 //     prologue (4 KB read), block 0 publishes the fp32 residual stream;
 //   * dot products follow the canonical order (lane l owns k = 256g + 8l + j; butterfly), identical
@@ -109,7 +112,7 @@ __global__ void __launch_bounds__(FG_THREADS) fast_gemv_kernel(FastArgs a) {
   __syncwarp();
   if (lane == 0 && wn > 0) {
     mbar_expect_tx(&sh.bar[warp], (uint32_t)wn * K * 2);
-    bulk_g2s(sw + (size_t)wr0 * K, a.W + (size_t)(row0 + wr0) * K, (uint32_t)wn * K * 2, &sh.bar[warp]);
+    bulk_g2s_evict_first(sw + (size_t)wr0 * K, a.W + (size_t)(row0 + wr0) * K, (uint32_t)wn * K * 2, &sh.bar[warp]);
   }
   // the other step-independent operands (bias, LayerNorm gamma / beta, the condition embedding) are loaded here too:
   // read after the wait they would each add a DRAM round trip, queued behind the weight streams, to the token's chain
