@@ -468,6 +468,29 @@ int ma_smooth_points(const float* xyz, int n, int k, float* out_xyz, float* norm
 void ma_smooth_points_set_events(void* const* events);
 void ma_smooth_points_set_order(int cell_order);
 
+/* ---- the colours of a scan carried onto a mesh (`--transfer_colors`; csrc/colors.cu) ---------------------------------
+ * vertices fp32 [V][3] and faces int32 [F][3] (indices in [0, V)) of the mesh, points fp32 [N][3] and colors fp32 [N][3]
+ * (in [0, 1]) of the scan, all finite and already in the points' frame -> out_colors fp32 [V][3], as DESIGN.md section
+ * 1.9 defines it: every point within r of the mesh adds its colour to the three corners of its nearest face (wt_tri_dist,
+ * the lowest face index on ties) with the barycentric weights of its nearest point there (wt_tri_bary), as unsigned
+ * 64-bit fixed-point sums W[v] += llrint(w 2^24), C[v][ch] += llrint(fl32(w c) 2^24); a vertex gets fl32(C / W) (fp64),
+ * or with W = 0 the colour of its nearest point (d^2 = (dx dx + dy dy) + dz dz, the lowest index on ties).  stats_out
+ * int64 [3] (device) = (points used, points beyond r, fallback vertices).  Optional test outputs (NULL: not written):
+ * point_face int32 [N] (the nearest face of every point), point_dist fp32 [N] (its distance), point_weights fp32 [N][3],
+ * sums_out uint64 [V][4] (W, C_r, C_g, C_b), fallback_out uint8 [V] (1 where W = 0).  1 <= V <= 196608,
+ * 1 <= F <= 65536 (every point is measured against every face), 1 <= N <= 2^24, 0 < r finite.  ws:
+ * ma_transfer_colors_workspace_bytes(V, F, N) bytes (0 for shapes out of range).  No host synchronisation and no
+ * floating-point atomics: two calls give identical bits. */
+size_t ma_transfer_colors_workspace_bytes(int V, int F, int N);
+int ma_transfer_colors(const float* vertices, int V, const int32_t* faces, int F, const float* points,
+                       const float* colors, int N, float r, float* out_colors, int64_t* stats_out, int32_t* point_face,
+                       float* point_dist, float* point_weights, uint64_t* sums_out, uint8_t* fallback_out, void* ws,
+                       void* stream);
+/* Measurement hook (tools/bench_colors.py): events = 4 cudaEvent_t recorded on the stream of every following call at its
+ * start and after the assignment, the accumulation and the fallback with the colours (NULL: off).  It changes no
+ * result. */
+void ma_transfer_colors_set_events(void* const* events);
+
 /* number of kernels launched by the library since load (bench.py's gpu_launches) */
 unsigned long long ma_launch_count(void);
 

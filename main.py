@@ -8,6 +8,8 @@
     python main.py --input_type pc --input_path scan.npy --smooth            # pull scanner noise back onto the surface
     python main.py --input_type pc --input_path scan.npy --remove_plane --split_objects --output_frame input
                                                    # one mesh per object on the table, each where it stands in the scan
+    python main.py --input_type pc --input_path scan.ply --remove_plane --transfer_colors
+                                                   # vertex colours of the mesh from the scan's red green blue
     torchrun --nproc-per-node 8 main.py --input_type pc_normal --input_dir pcs --batchsize_per_gpu 64
 
 Differences forced by the environment: no accelerate / hf_hub (there is no network) -- one process per
@@ -101,7 +103,21 @@ def _farthest_points(xyz, path, n_points=4096):
     return idx.cpu().numpy()
 
 
-def _subsample_points(path, n_points=4096, outliers=None, subsample='random', plane=None, objects=None, smooth=None):
+def _rows(a, idx):
+    """a[idx], or None for None: the colours of a cloud follow its rows through every stage that drops rows."""
+    return None if a is None else a[idx]
+
+
+def _colored(cloud, xyz, rgb):
+    """cloud, or with rgb (`--transfer_colors`) (cloud, the full cleaned cloud float64 [M, 6]: xyz in the input's units |
+    rgb), which the generated mesh takes its colours from."""
+    if rgb is None:
+        return cloud
+    return cloud, np.concatenate([np.asarray(xyz, dtype=np.float64), np.asarray(rgb, dtype=np.float64)], axis=1)
+
+
+def _subsample_points(path, n_points=4096, outliers=None, subsample='random', plane=None, objects=None, smooth=None,
+                      colors=False):
     """`--input_type pc_normal`: an .npy of >= 4096 (xyz, normal) rows; a random 4096-subset without replacement
     (global numpy RNG, seeded by --seed as the reference does through accelerate.set_seed), or with
     subsample='fps' the farthest-point subset of the xyz columns.  With `outliers` (the keyword arguments of
@@ -109,20 +125,29 @@ def _subsample_points(path, n_points=4096, outliers=None, subsample='random', pl
     arguments of meshanything_b200.plane.remove_plane) the support plane goes before that.  With `smooth` ({'k': k})
     the xyz columns of the cleaned rows are smoothed; the normals pass through unchanged.  With `objects` ({'distance':
     e}) the cleaned cloud is split into objects and a list of one subset per object is returned, drawn in object
-    order."""
-    cloud = np.load(path)
+    order.  With `colors` the file is (N, 9), xyz | normal | rgb: the colours follow their rows, and every subset comes
+    with its full cleaned cloud (see _colored)."""
+    cloud, rgb = np.load(path), None
+    if colors:
+        if cloud.ndim != 2 or cloud.shape[1] != 9:
+            raise ValueError(f"{path}: --transfer_colors reads a coloured pc_normal cloud as an array of shape (N, 9), "
+                             f"xyz | normal | rgb, got {cloud.shape}")
+        from mesh_to_pc import check_rgb
+        cloud, rgb = cloud[:, :6], check_rgb(path, cloud[:, 6:])
     if plane is not None:
-        cloud = cloud[_remove_plane(cloud[:, :3], path, plane, n_points)]
+        keep = _remove_plane(cloud[:, :3], path, plane, n_points)
+        cloud, rgb = cloud[keep], _rows(rgb, keep)
     if outliers is not None:
-        cloud = cloud[_remove_outliers(cloud[:, :3], path, outliers, n_points)]
+        keep = _remove_outliers(cloud[:, :3], path, outliers, n_points)
+        cloud, rgb = cloud[keep], _rows(rgb, keep)
     if smooth is not None:
         cloud = cloud.copy()
         cloud[:, :3] = _smooth(cloud[:, :3], path, smooth)
     assert cloud.shape[0] >= n_points, "input pc_normal should have at least 4096 points"
     if objects is not None:
-        return [_subset(cloud[part], path, n_points, subsample)
+        return [_colored(_subset(cloud[part], path, n_points, subsample), cloud[part, :3], _rows(rgb, part))
                 for part in _split_objects(cloud[:, :3], path, objects, n_points)]
-    return _subset(cloud, path, n_points, subsample)
+    return _colored(_subset(cloud, path, n_points, subsample), cloud[:, :3], rgb)
 
 
 def _subset(cloud, path, n_points, subsample):
@@ -134,7 +159,7 @@ def _subset(cloud, path, n_points, subsample):
 
 
 def _points_with_normals(path, n_points=4096, k=16, outliers=None, subsample='random', plane=None, objects=None,
-                         smooth=None):
+                         smooth=None, colors=False):
     """`--input_type pc`: a bare cloud (.npy (N, 3) or vertex-only .ply) of >= 4096 points.  Normals are estimated on
     the GPU from all N points (meshanything_b200.normals), then the same 4096-subset as `pc_normal` is drawn: the
     xyz-only copy of a file selects the points the file with normals selects under the same seed.  With `outliers`
@@ -142,22 +167,25 @@ def _points_with_normals(path, n_points=4096, k=16, outliers=None, subsample='ra
     before that; `smooth` smooths the cleaned points before their normals are estimated.  With `objects` the cleaned
     cloud is split into objects first, and every object gets its own normals (estimated on its points alone, so that
     their orientation is rooted at its own farthest point) and subset, in object order: a list of one cloud per object
-    is returned."""
+    is returned.  With `colors` the file carries rgb (mesh_to_pc.load_points): the colours follow their rows, and every
+    cloud comes with its full cleaned cloud (see _colored)."""
     from mesh_to_pc import load_points
-    xyz = load_points(path)
+    xyz, rgb = load_points(path, colors=True) if colors else (load_points(path), None)
     if not np.issubdtype(xyz.dtype, np.floating):
         xyz = xyz.astype(np.float64)
     assert xyz.shape[0] >= n_points, "input pc_normal should have at least 4096 points"
     if plane is not None:
-        xyz = xyz[_remove_plane(xyz, path, plane, n_points)]
+        keep = _remove_plane(xyz, path, plane, n_points)
+        xyz, rgb = xyz[keep], _rows(rgb, keep)
     if outliers is not None:
-        xyz = xyz[_remove_outliers(xyz, path, outliers, n_points)]
+        keep = _remove_outliers(xyz, path, outliers, n_points)
+        xyz, rgb = xyz[keep], _rows(rgb, keep)
     if smooth is not None:
         xyz = _smooth(xyz, path, smooth)
     if objects is not None:
-        return [_with_normals(xyz[part], path, n_points, k, subsample)
+        return [_colored(_with_normals(xyz[part], path, n_points, k, subsample), xyz[part], _rows(rgb, part))
                 for part in _split_objects(xyz, path, objects, n_points)]
-    return _with_normals(xyz, path, n_points, k, subsample)
+    return _colored(_with_normals(xyz, path, n_points, k, subsample), xyz, rgb)
 
 
 def _with_normals(xyz, path, n_points, k, subsample):
@@ -169,6 +197,24 @@ def _with_normals(xyz, path, n_points, k, subsample):
     else:
         keep = np.random.choice(xyz.shape[0], n_points, replace=False)
     return np.concatenate([xyz[keep], normals[keep].astype(xyz.dtype)], axis=1)
+
+
+def _vertex_colors(item, vertices, faces, output_frame, distance):
+    """`--transfer_colors`: rgb [V, 3] of the final mesh (vertices in the output frame) from the item's full cleaned
+    cloud (DESIGN.md section 1.9, on the GPU, meshanything_b200.colors).  The mesh is first put in the input's units
+    (metrics.to_input_frame), so that both output frames give the same colours; one line per item with the counts."""
+    from meshanything_b200.colors import transfer_colors
+    from meshanything_b200.metrics import to_input_frame
+    if len(faces) == 0:
+        return np.zeros((len(vertices), 3))
+    v = torch.as_tensor(np.asarray(vertices, dtype=np.float64))
+    if output_frame == 'model':
+        v = to_input_frame(v, item['frame'])
+    cloud = item['colors']
+    rgb, st = transfer_colors(v, np.asarray(faces, dtype=np.int64), cloud[:, :3], cloud[:, 3:], distance)
+    print(f"{item['uid']}: coloured {len(v)} vertices from {st.used} of {st.n_points} points ({st.beyond} farther than "
+          f"{distance:g} of the cloud's longest side); {st.fallback_vertices} vertices took their nearest point's colour")
+    return rgb.cpu().numpy()
 
 
 def _uid_of(path):
@@ -183,6 +229,8 @@ _NO_MESH_OBJECTS = ("--split_objects applies to point-cloud input (--input_type 
                     "its connected parts is not supported")
 _NO_MESH_SMOOTH = ("--smooth applies to point-cloud input (--input_type pc or pc_normal): the points of a mesh are "
                    "sampled exactly from its surface and carry no scanner noise")
+_NO_MESH_COLORS = ("--transfer_colors applies to point-cloud input (--input_type pc or pc_normal): colours of a mesh's "
+                   "own vertices or textures are not read")
 _NO_MESH_PLANE = ("--remove_plane applies to point-cloud input (--input_type pc or pc_normal): the points of a mesh are "
                   "sampled from its own surface, which has no scanned support under it")
 SUBSAMPLERS = ('random', 'fps')
@@ -208,10 +256,12 @@ class Dataset:
     {'k': k}, to smooth every cloud after plane and outlier removal (DESIGN.md section 1.8; for pc_normal only the xyz
     columns move).  Items also carry 'frame', the
     metrics.shape_frame of the rows before normalisation, which metrics.to_input_frame applies to put a mesh back in
-    the input's coordinates."""
+    the input's coordinates.  `colors` (point clouds only, `--transfer_colors`): read the files' colours, and give every
+    item a 'colors' entry, float64 [M, 6]: the full cleaned cloud it was drawn from (after plane and outlier removal,
+    smoothing and splitting; not the 4096-point subset), xyz in the input's units | rgb in [0, 1]."""
 
     def __init__(self, input_type, input_list, mc=False, outliers=None, subsample='random', plane=None, objects=None,
-                 smooth=None):
+                 smooth=None, colors=False):
         if outliers is not None and input_type not in ('pc', 'pc_normal'):
             raise ValueError(_NO_MESH_OUTLIERS)
         if plane is not None and input_type not in ('pc', 'pc_normal'):
@@ -220,10 +270,14 @@ class Dataset:
             raise ValueError(_NO_MESH_OBJECTS)
         if smooth is not None and input_type not in ('pc', 'pc_normal'):
             raise ValueError(_NO_MESH_SMOOTH)
+        if colors and input_type not in ('pc', 'pc_normal'):
+            raise ValueError(_NO_MESH_COLORS)
         _check_subsample(input_type, subsample)
         kw = dict(outliers=outliers, subsample=subsample, plane=plane, objects=objects)
         if smooth is not None:
             kw['smooth'] = smooth
+        if colors:
+            kw['colors'] = True
         if input_type == 'pc_normal':
             clouds = [_subsample_points(p, **kw) for p in input_list]
         elif input_type == 'pc':
@@ -239,6 +293,9 @@ class Dataset:
         else:
             self.data = [{'pc_normal': c, 'uid': f"{_uid_of(p)}_obj{k}"}
                          for cs, p in zip(clouds, input_list) for k, c in enumerate(cs)]
+        if colors:
+            for entry in self.data:
+                entry['pc_normal'], entry['colors'] = entry['pc_normal']
         print(f"dataset total data samples: {len(self.data)}")
 
     def __len__(self):
@@ -248,8 +305,11 @@ class Dataset:
         from meshanything_b200.inputs import normalize_pc_normal
         from meshanything_b200.metrics import shape_frame
         entry = self.data[idx]
-        return {'pc_normal': normalize_pc_normal(entry['pc_normal']), 'uid': entry['uid'],
+        item = {'pc_normal': normalize_pc_normal(entry['pc_normal']), 'uid': entry['uid'],
                 'frame': shape_frame(entry['pc_normal'][:, :3])}
+        if 'colors' in entry:
+            item['colors'] = entry['colors']
+        return item
 
 
 _FLAGS = [  # (flag, default, type) -- the reference's command line (main.py:60-89)
@@ -306,6 +366,15 @@ def get_args():
     # not in the reference: write meshes in the model's [-0.5, 0.5) frame (model, the reference's output) or back in
     # the input's coordinates (input: c + L v with the bounding box centre c and longest side L of the shape's points)
     parser.add_argument('--output_frame', default='model', choices=OUTPUT_FRAMES)
+    # not in the reference: colour the mesh's vertices from the scan's per-point red green blue (a .ply with colour
+    # properties, an (N, 6) xyz | rgb .npy for pc, an (N, 9) xyz | normal | rgb .npy for pc_normal) instead of the
+    # constant orange; points farther than --color_distance of the cloud's longest side from the mesh are ignored
+    # (DESIGN.md section 1.9; meshanything_b200.colors)
+    parser.add_argument('--transfer_colors', default=False, action="store_true",
+                        help="colour the mesh's vertices from the scan's per-point colours (point-cloud input)")
+    parser.add_argument('--color_distance', default=0.05, type=float,
+                        help="points farther than this share of the cloud's longest side from the mesh give no colour, "
+                             "in (0, 1] (default 0.05)")
     return parser.parse_args()
 
 
@@ -336,6 +405,11 @@ def smooth_options(args):
     if not getattr(args, 'smooth', False):
         return None
     return {'k': getattr(args, 'smooth_neighbors', 24)}
+
+
+def color_options(args):
+    """The `colors` argument of Dataset from the command line."""
+    return bool(getattr(args, 'transfer_colors', False))
 
 
 def check_args(args):
@@ -378,6 +452,13 @@ def check_args(args):
         k = getattr(args, 'smooth_neighbors', 24)
         if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 5 <= k <= 64:
             raise ValueError(f"--smooth_neighbors must be in 5..64, got {k}")
+    if getattr(args, 'transfer_colors', False):
+        if args.input_type == 'mesh':
+            raise ValueError(_NO_MESH_COLORS)
+        distance = getattr(args, 'color_distance', 0.05)
+        if not (np.isfinite(distance) and 0 < distance <= 1 and np.float32(distance) > 0):
+            raise ValueError(f"--color_distance must be in (0, 1] (a share of the bounding box's longest side), got "
+                             f"{distance}")
     if getattr(args, 'output_frame', 'model') not in OUTPUT_FRAMES:
         raise ValueError(f"--output_frame must be one of {', '.join(OUTPUT_FRAMES)}, got {args.output_frame!r}")
 
@@ -449,9 +530,10 @@ def fix_winding(vertices, tri):
     return tri
 
 
-def export_obj(path, faces_xyz):
+def export_obj(path, faces_xyz, vertex_colors=None):
     """merge_vertices + unique_faces + fix_normals + orange face colour of main.py:161-174 (trimesh when available,
-    the numpy equivalents otherwise)."""
+    the numpy equivalents otherwise).  With `vertex_colors`, a function of the final (vertices float64 [V, 3], faces
+    int64 [F, 3]) returning rgb [V, 3] in [0, 1], the vertices get those colours instead of the orange."""
     vertices = faces_xyz.reshape(-1, 3)
     triangles = np.arange(len(vertices)).reshape(-1, 3)
     try:
@@ -460,7 +542,13 @@ def export_obj(path, faces_xyz):
         mesh.merge_vertices()
         mesh.update_faces(mesh.unique_faces())
         mesh.fix_normals()
-        mesh.visual.face_colors = np.tile(np.array([255, 165, 0, 255], dtype=np.uint8), (len(mesh.faces), 1))
+        if vertex_colors is None:
+            mesh.visual.face_colors = np.tile(np.array([255, 165, 0, 255], dtype=np.uint8), (len(mesh.faces), 1))
+        else:
+            rgb = np.asarray(vertex_colors(np.asarray(mesh.vertices, dtype=np.float64),
+                                           np.asarray(mesh.faces, dtype=np.int64)), dtype=np.float64)
+            mesh.visual.vertex_colors = np.concatenate(
+                [np.round(rgb * 255).astype(np.uint8), np.full((len(rgb), 1), 255, np.uint8)], axis=1)
         mesh.export(path)
         return len(mesh.faces)
     except ImportError:
@@ -468,9 +556,13 @@ def export_obj(path, faces_xyz):
         tri = inv.reshape(-1)[triangles]
         _, keep = np.unique(np.sort(tri, axis=1), axis=0, return_index=True)
         tri = fix_winding(uniq, tri[np.sort(keep)])
+        rgb = None if vertex_colors is None else np.asarray(vertex_colors(uniq, tri), dtype=np.float64)
         with open(path, "w") as f:
-            for v in uniq:
-                f.write(f"v {v[0]:.8f} {v[1]:.8f} {v[2]:.8f} 1.00000000 0.64705882 0.00000000\n")
+            for k, v in enumerate(uniq):
+                if rgb is None:
+                    f.write(f"v {v[0]:.8f} {v[1]:.8f} {v[2]:.8f} 1.00000000 0.64705882 0.00000000\n")
+                else:
+                    f.write(f"v {v[0]:.8f} {v[1]:.8f} {v[2]:.8f} {rgb[k, 0]:.8f} {rgb[k, 1]:.8f} {rgb[k, 2]:.8f}\n")
             for t in tri:
                 f.write(f"f {t[0] + 1} {t[1] + 1} {t[2] + 1}\n")
         return len(tri)
@@ -504,7 +596,8 @@ if __name__ == "__main__":
     np.random.seed(args.seed)
     torch.manual_seed(args.seed)
     dataset = Dataset(args.input_type, input_list, args.mc, outliers=outlier_options(args), subsample=args.subsample,
-                      plane=plane_options(args), objects=object_options(args), smooth=smooth_options(args))
+                      plane=plane_options(args), objects=object_options(args), smooth=smooth_options(args),
+                      colors=color_options(args))
 
     bs = args.batchsize_per_gpu
     batches = [list(range(i, min(i + bs, len(dataset)))) for i in range(0, len(dataset), bs)]
@@ -517,7 +610,11 @@ if __name__ == "__main__":
             from meshanything_b200.metrics import to_input_frame
             recon_mesh = to_input_frame(recon_mesh, item['frame'])
         save_path = os.path.join(checkpoint_dir, f'{item["uid"]}_gen.obj')
-        export_obj(save_path, recon_mesh.cpu().numpy())
+        colors = None
+        if 'colors' in item:
+            def colors(vertices, faces):
+                return _vertex_colors(item, vertices, faces, args.output_frame, args.color_distance)
+        export_obj(save_path, recon_mesh.cpu().numpy(), colors)
         print(f"{save_path} Over!!")
 
     if args.continuous_batching:

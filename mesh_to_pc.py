@@ -74,8 +74,10 @@ class SimpleMesh:
         return SimpleMesh(verts, np.asarray(faces, dtype=np.int64))
 
     @staticmethod
-    def _read_ply(path):
-        """(vertices float64 [V, 3] or None, list of triangles) of a PLY file."""
+    def _read_ply(path, colors=False):
+        """(vertices float64 [V, 3] or None, list of triangles) of a PLY file; with `colors` also the vertices' `red
+        green blue` as float64 [V, 3] (integer types divided by their maximum, float types as stored; ValueError when
+        they are missing or outside [0, 1])."""
         T = SimpleMesh._PLY_TYPES
         with open(path, "rb") as f:
             if f.readline().strip() != b"ply":
@@ -102,7 +104,7 @@ class SimpleMesh:
             if fmt not in ("ascii", "binary_little_endian", "binary_big_endian"):
                 raise ValueError(f"{path}: unsupported PLY format {fmt!r}")
             end = ">" if fmt == "binary_big_endian" else "<"
-            verts, faces = None, []
+            verts, faces, rgb = None, [], None
             for el in elements:
                 n, props = el["count"], el["props"]
                 has_list = any(pr[0] == "list" for pr in props)
@@ -112,6 +114,10 @@ class SimpleMesh:
                         names = [pr[1] for pr in props]
                         ix = [names.index(c) for c in "xyz"]
                         verts = np.array([[float(r[i]) for i in ix] for r in rows], dtype=np.float64).reshape(-1, 3)
+                        if colors:
+                            ic = _rgb_columns(path, names)
+                            rgb = np.array([[float(r[i]) for i in ic] for r in rows], dtype=np.float64).reshape(-1, 3)
+                            rgb = _scale_rgb(path, rgb, [props[i][2] for i in ic])
                     elif el["name"] == "face":
                         for r in rows:   # list property first (the usual layout); scalar face properties follow it
                             k = int(r[0])
@@ -123,6 +129,10 @@ class SimpleMesh:
                     block = np.frombuffer(f.read(dt.itemsize * n), dtype=dt, count=n)
                     if el["name"] == "vertex":
                         verts = np.stack([block[c].astype(np.float64) for c in "xyz"], axis=1)
+                        if colors:
+                            ic = _rgb_columns(path, [pr[1] for pr in props])
+                            rgb = np.stack([block[props[i][1]].astype(np.float64) for i in ic], axis=1)
+                            rgb = _scale_rgb(path, rgb, [props[i][2] for i in ic])
                     continue
                 for _ in range(n):       # element with a list property: variable-length records
                     for pr in props:
@@ -133,14 +143,63 @@ class SimpleMesh:
                         ids = np.frombuffer(f.read(np.dtype(pr[3]).itemsize * k), dtype=end + pr[3]).astype(np.int64)
                         if el["name"] == "face":
                             faces.extend([ids[0], ids[j], ids[j + 1]] for j in range(1, k - 1))
+        if colors:
+            if verts is not None and rgb is None:
+                raise ValueError(f"{path}: PLY vertices without red, green and blue properties (--transfer_colors "
+                                 "needs the scan's colours)")
+            return verts, faces, rgb
         return verts, faces
 
 
-def load_points(path):
+_RGB = ("red", "green", "blue")
+
+
+def _rgb_columns(path, names):
+    """Indices of red, green, blue among a vertex element's property names (alpha and the others are ignored)."""
+    if not all(c in names for c in _RGB):
+        raise ValueError(f"{path}: PLY vertices without red, green and blue properties (--transfer_colors needs the "
+                         "scan's colours)")
+    return [names.index(c) for c in _RGB]
+
+
+def _scale_rgb(path, rgb, types):
+    """PLY colour columns to [0, 1]: integer types divided by their maximum (255 for uchar), float types as stored."""
+    for k, t in enumerate(types):
+        if np.dtype(t).kind in "iu":
+            rgb[:, k] /= np.iinfo(np.dtype(t)).max
+    return check_rgb(path, rgb)
+
+
+def check_rgb(path, rgb):
+    """rgb [N, 3] float64, or ValueError unless every value is finite and in [0, 1]."""
+    rgb = np.asarray(rgb, dtype=np.float64)
+    if not np.all(np.isfinite(rgb) & (rgb >= 0) & (rgb <= 1)):
+        raise ValueError(f"{path}: colours outside [0, 1] (integer colours are divided by their type's maximum, float "
+                         "colours are taken as stored)")
+    return rgb
+
+
+def load_points(path, colors=False):
     """A bare point cloud for `--input_type pc`: an .npy of shape (N, 3), or a .ply with a `vertex` element (x, y, z
     among any other properties; ASCII or binary) and no faces.  Returns the xyz array ([N, 3]; the .npy's own dtype,
-    float64 from a PLY).  An (N, 6) .npy is refused rather than having its normals dropped."""
+    float64 from a PLY).  An (N, 6) .npy is refused rather than having its normals dropped.
+
+    With `colors` (`--transfer_colors`) returns (xyz, rgb float64 [N, 3] in [0, 1]) instead: an .npy of shape (N, 6),
+    xyz | rgb, or a .ply whose vertices carry `red green blue` (see SimpleMesh._read_ply)."""
     low = path.lower()
+    if colors and low.endswith(".npy"):
+        cloud = np.load(path)
+        if cloud.ndim != 2 or cloud.shape[1] != 6:
+            raise ValueError(f"{path}: --transfer_colors reads a coloured point cloud as an array of shape (N, 6), "
+                             f"xyz | rgb, got {cloud.shape}")
+        return cloud[:, :3], check_rgb(path, cloud[:, 3:])
+    if colors and low.endswith(".ply"):
+        verts, faces, rgb = SimpleMesh._read_ply(path, colors=True)
+        if verts is None:
+            raise ValueError(f"{path}: PLY without a vertex element")
+        if faces:
+            raise ValueError(f"{path}: PLY with faces is a mesh; use --input_type mesh")
+        return verts, rgb
     if low.endswith(".npy"):
         xyz = np.load(path)
         if xyz.ndim == 2 and xyz.shape[1] == 6:

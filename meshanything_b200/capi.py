@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import ctypes as C
 import math
+import numbers
 import operator
 import os
 from typing import Optional
@@ -56,6 +57,7 @@ EXPORTS = [
     "ma_remove_plane_workspace_bytes", "ma_remove_plane", "ma_remove_plane_set_events",
     "ma_split_objects_workspace_bytes", "ma_split_objects", "ma_split_objects_set_events",
     "ma_smooth_points_workspace_bytes", "ma_smooth_points", "ma_smooth_points_set_events", "ma_smooth_points_set_order",
+    "ma_transfer_colors_workspace_bytes", "ma_transfer_colors", "ma_transfer_colors_set_events",
     "ma_fourier_embed_f16", "ma_scatter_heads_f16", "ma_residual_add", "ma_convert_rows", "ma_add_table",
     "ma_gather_codes", "ma_coords",
 ]
@@ -170,6 +172,12 @@ def lib():
     L.ma_smooth_points_set_events.restype = None
     L.ma_smooth_points_set_order.argtypes = [C.c_int]
     L.ma_smooth_points_set_order.restype = None
+    L.ma_transfer_colors_workspace_bytes.argtypes = [C.c_int, C.c_int, C.c_int]
+    L.ma_transfer_colors_workspace_bytes.restype = C.c_size_t
+    L.ma_transfer_colors.argtypes = [_vp, C.c_int, _vp, C.c_int, _vp, _vp, C.c_int, C.c_float, _vp, _vp, _vp, _vp, _vp,
+                                     _vp, _vp, _vp, _vp]
+    L.ma_transfer_colors_set_events.argtypes = [_vp]
+    L.ma_transfer_colors_set_events.restype = None
     L.ma_fourier_embed_f16.argtypes = [_vp, C.c_long, _vp, _vp]
     L.ma_scatter_heads_f16.argtypes = [_vp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_long, _vp, C.c_long, _vp]
     L.ma_residual_add.argtypes = [_vp, _vp, _vp, C.c_long, _vp]
@@ -630,6 +638,69 @@ def smooth_points(points: torch.Tensor, k: int = 24, want_terms: bool = False):
                                      ptr(ws), stream_ptr()), "ma_smooth_points")
         st = stats.cpu().numpy()
     return (out, st, normals, flags, knn) if want_terms else (out, st)
+
+
+COLORS_MAX_F = 1 << 16
+COLORS_MAX_V = 3 * COLORS_MAX_F
+
+
+def transfer_colors(vertices: torch.Tensor, faces: torch.Tensor, points: torch.Tensor, colors: torch.Tensor,
+                    r: float, want_terms: bool = False):
+    """The colours of a scan carried onto a mesh (ma_transfer_colors; colors.transfer_colors adds the frame map).
+
+    vertices fp32 [V, 3] and points fp32 [N, 3], finite and already in the points' frame; faces int32 [F, 3] with
+    indices in [0, V); colors fp32 [N, 3] in [0, 1]; all contiguous on one CUDA device; 1 <= V <= 196608,
+    1 <= F <= 65536, 1 <= N <= 2^24; r > 0 finite (rounded to fp32, which must stay > 0).  Returns (vertex colours fp32
+    [V, 3], stats int64 [3] on the host: points used, points beyond r, fallback vertices); with want_terms also (nearest
+    face int32 [N], its distance fp32 [N], weights fp32 [N, 3], sums uint64 as int64 [V, 4] = W, C_r, C_g, C_b, fallback
+    flags uint8 [V]).  Every bad input raises ValueError before anything is launched.  Reads the stats back
+    (synchronises)."""
+    what = "transfer_colors"
+    n = _check_points(what, points, 1)
+    dev = points.device
+    for name, t, rows in (("vertices", vertices, None), ("colors", colors, n)):
+        if not isinstance(t, torch.Tensor):
+            raise ValueError(f"{what}: {name} must be a torch tensor, got {type(t).__name__}")
+        if t.dim() != 2 or t.shape[1] != 3 or (rows is not None and t.shape[0] != rows):
+            raise ValueError(f"{what}: {name} [{'N' if rows else 'V'}, 3], got {tuple(t.shape)}")
+        if t.dtype != torch.float32 or not t.is_contiguous() or t.device != dev:
+            raise ValueError(f"{what}: {name} must be contiguous float32 on {dev}, got {t.dtype} on {t.device}")
+        if not bool(torch.isfinite(t).all()):
+            raise ValueError(f"{what}: non-finite {name}")
+    if not bool(((colors >= 0) & (colors <= 1)).all()):
+        raise ValueError(f"{what}: colors outside [0, 1]")
+    V = vertices.shape[0]
+    if not 1 <= V <= COLORS_MAX_V:
+        raise ValueError(f"{what}: 1 <= V <= {COLORS_MAX_V}, got V = {V}")
+    if not isinstance(faces, torch.Tensor):
+        raise ValueError(f"{what}: faces must be a torch tensor, got {type(faces).__name__}")
+    if faces.dim() != 2 or faces.shape[1] != 3:
+        raise ValueError(f"{what}: faces [F, 3], got {tuple(faces.shape)}")
+    if faces.dtype != torch.int32 or not faces.is_contiguous() or faces.device != dev:
+        raise ValueError(f"{what}: faces must be contiguous int32 on {dev}, got {faces.dtype} on {faces.device}")
+    F = faces.shape[0]
+    if not 1 <= F <= COLORS_MAX_F:
+        raise ValueError(f"{what}: 1 <= F <= {COLORS_MAX_F}, got F = {F}")
+    if int(faces.min()) < 0 or int(faces.max()) >= V:
+        raise ValueError(f"{what}: face indices outside [0, {V})")
+    if isinstance(r, bool) or not isinstance(r, numbers.Real):
+        raise ValueError(f"{what}: r must be a real number, got {r!r}")
+    r = float(r)
+    r32 = C.c_float(r).value
+    if not (math.isfinite(r) and math.isfinite(r32) and r32 > 0):
+        raise ValueError(f"{what}: r > 0 and finite (also in fp32), got {r}")
+    ws = torch.empty(lib().ma_transfer_colors_workspace_bytes(V, F, n), dtype=torch.uint8, device=dev)
+    out = torch.empty((V, 3), dtype=torch.float32, device=dev)
+    stats = torch.empty((3,), dtype=torch.int64, device=dev)
+    extra = (torch.empty((n,), dtype=torch.int32, device=dev), torch.empty((n,), dtype=torch.float32, device=dev),
+             torch.empty((n, 3), dtype=torch.float32, device=dev), torch.empty((V, 4), dtype=torch.int64, device=dev),
+             torch.empty((V,), dtype=torch.uint8, device=dev)) if want_terms else (None,) * 5
+    with torch.cuda.device(dev):
+        check(lib().ma_transfer_colors(ptr(vertices), V, ptr(faces), F, ptr(points), ptr(colors), n, C.c_float(r32),
+                                       ptr(out), ptr(stats), *[ptr(t) for t in extra], ptr(ws), stream_ptr()),
+              "ma_transfer_colors")
+        st = stats.cpu().numpy()
+    return (out, st, *extra) if want_terms else (out, st)
 
 
 def tensor_core_linear_counts():
