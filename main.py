@@ -21,12 +21,14 @@ import argparse
 import datetime
 import os
 import time
+from typing import Callable, NamedTuple
 
 import numpy as np
 import torch
 
 from MeshAnything.models.meshanything import MeshAnything
-from mesh_to_pc import load_mesh, process_mesh_to_pc
+from mesh_to_pc import load_cloud, load_mesh, process_mesh_to_pc
+from meshanything_b200 import capi
 
 
 def _remove_outliers(xyz, path, outliers, n_points=4096):
@@ -103,100 +105,44 @@ def _farthest_points(xyz, path, n_points=4096):
     return idx.cpu().numpy()
 
 
-def _rows(a, idx):
-    """a[idx], or None for None: the colours of a cloud follow its rows through every stage that drops rows."""
-    return None if a is None else a[idx]
-
-
-def _colored(cloud, xyz, rgb):
-    """cloud, or with rgb (`--transfer_colors`) (cloud, the full cleaned cloud float64 [M, 6]: xyz in the input's units |
-    rgb), which the generated mesh takes its colours from."""
-    if rgb is None:
-        return cloud
-    return cloud, np.concatenate([np.asarray(xyz, dtype=np.float64), np.asarray(rgb, dtype=np.float64)], axis=1)
-
-
-def _subsample_points(path, n_points=4096, outliers=None, subsample='random', plane=None, objects=None, smooth=None,
-                      colors=False):
-    """`--input_type pc_normal`: an .npy of >= 4096 (xyz, normal) rows; a random 4096-subset without replacement
-    (global numpy RNG, seeded by --seed as the reference does through accelerate.set_seed), or with
-    subsample='fps' the farthest-point subset of the xyz columns.  With `outliers` (the keyword arguments of
-    meshanything_b200.outliers.remove_outliers) the rows are first cleaned by their xyz; with `plane` (the keyword
-    arguments of meshanything_b200.plane.remove_plane) the support plane goes before that.  With `smooth` ({'k': k})
-    the xyz columns of the cleaned rows are smoothed; the normals pass through unchanged.  With `objects` ({'distance':
-    e}) the cleaned cloud is split into objects and a list of one subset per object is returned, drawn in object
-    order.  With `colors` the file is (N, 9), xyz | normal | rgb: the colours follow their rows, and every subset comes
-    with its full cleaned cloud (see _colored)."""
-    cloud, rgb = np.load(path), None
-    if colors:
-        if cloud.ndim != 2 or cloud.shape[1] != 9:
-            raise ValueError(f"{path}: --transfer_colors reads a coloured pc_normal cloud as an array of shape (N, 9), "
-                             f"xyz | normal | rgb, got {cloud.shape}")
-        from mesh_to_pc import check_rgb
-        cloud, rgb = cloud[:, :6], check_rgb(path, cloud[:, 6:])
-    if plane is not None:
-        keep = _remove_plane(cloud[:, :3], path, plane, n_points)
-        cloud, rgb = cloud[keep], _rows(rgb, keep)
-    if outliers is not None:
-        keep = _remove_outliers(cloud[:, :3], path, outliers, n_points)
-        cloud, rgb = cloud[keep], _rows(rgb, keep)
-    if smooth is not None:
-        cloud = cloud.copy()
-        cloud[:, :3] = _smooth(cloud[:, :3], path, smooth)
-    assert cloud.shape[0] >= n_points, "input pc_normal should have at least 4096 points"
-    if objects is not None:
-        return [_colored(_subset(cloud[part], path, n_points, subsample), cloud[part, :3], _rows(rgb, part))
-                for part in _split_objects(cloud[:, :3], path, objects, n_points)]
-    return _colored(_subset(cloud, path, n_points, subsample), cloud[:, :3], rgb)
-
-
-def _subset(cloud, path, n_points, subsample):
-    """The 4096 rows of a cloud the model sees: random without replacement (global numpy RNG) or farthest points."""
-    if subsample == 'fps':
-        return cloud[_farthest_points(cloud[:, :3], path, n_points)]
-    keep = np.random.choice(cloud.shape[0], n_points, replace=False)
-    return cloud[keep]
-
-
-def _points_with_normals(path, n_points=4096, k=16, outliers=None, subsample='random', plane=None, objects=None,
-                         smooth=None, colors=False):
-    """`--input_type pc`: a bare cloud (.npy (N, 3) or vertex-only .ply) of >= 4096 points.  Normals are estimated on
-    the GPU from all N points (meshanything_b200.normals), then the same 4096-subset as `pc_normal` is drawn: the
-    xyz-only copy of a file selects the points the file with normals selects under the same seed.  With `outliers`
-    the cloud is cleaned first, and normals and subset come from the kept points; `plane` removes the support plane
-    before that; `smooth` smooths the cleaned points before their normals are estimated.  With `objects` the cleaned
-    cloud is split into objects first, and every object gets its own normals (estimated on its points alone, so that
-    their orientation is rooted at its own farthest point) and subset, in object order: a list of one cloud per object
-    is returned.  With `colors` the file carries rgb (mesh_to_pc.load_points): the colours follow their rows, and every
-    cloud comes with its full cleaned cloud (see _colored)."""
-    from mesh_to_pc import load_points
-    xyz, rgb = load_points(path, colors=True) if colors else (load_points(path), None)
-    if not np.issubdtype(xyz.dtype, np.floating):
-        xyz = xyz.astype(np.float64)
-    assert xyz.shape[0] >= n_points, "input pc_normal should have at least 4096 points"
-    if plane is not None:
-        keep = _remove_plane(xyz, path, plane, n_points)
-        xyz, rgb = xyz[keep], _rows(rgb, keep)
-    if outliers is not None:
-        keep = _remove_outliers(xyz, path, outliers, n_points)
-        xyz, rgb = xyz[keep], _rows(rgb, keep)
+def _cloud_items(input_type, path, outliers=None, subsample='random', plane=None, objects=None, smooth=None,
+                 colors=False, n_points=4096, k=16):
+    """The Dataset entries of one point-cloud file (mesh_to_pc.load_cloud), its stages in this order: `plane` removes
+    the support plane, `outliers` the stray points, `smooth` moves the xyz of the rest onto their surface (a pc_normal
+    file's normals pass through unchanged), and `objects` splits it into objects, each its own entry with uid
+    `{uid}_obj{k}`.  A stage that drops points drops the same rows of the file's normals and colours.  Then, object by
+    object: a bare cloud (`pc`) gets normals estimated on the GPU from that object's points alone
+    (meshanything_b200.normals), so that their orientation is rooted at its own farthest point, and the 4096 rows the
+    model sees are drawn at random without replacement (global numpy RNG, seeded by --seed as the reference does
+    through accelerate.set_seed), or with subsample='fps' by farthest-point sampling; the xyz-only copy of a file
+    selects the points the file with normals selects under the same seed.  With `colors` every entry also gets
+    'colors', float64 [M, 6]: the object's full cloud, xyz in the input's units | rgb, which the generated mesh takes
+    its colours from."""
+    from meshanything_b200.normals import estimate_normals
+    xyz, normals, rgb = load_cloud(path, input_type, colors)
+    if input_type == 'pc':   # a bare cloud is refused before its stages, one with normals after the ones that clean it
+        assert xyz.shape[0] >= n_points, "input pc_normal should have at least 4096 points"
+    for stage, options in ((_remove_plane, plane), (_remove_outliers, outliers)):
+        if options is not None:
+            keep = stage(xyz, path, options, n_points)
+            xyz, normals, rgb = (None if a is None else a[keep] for a in (xyz, normals, rgb))
     if smooth is not None:
         xyz = _smooth(xyz, path, smooth)
-    if objects is not None:
-        return [_colored(_with_normals(xyz[part], path, n_points, k, subsample), xyz[part], _rows(rgb, part))
-                for part in _split_objects(xyz, path, objects, n_points)]
-    return _colored(_with_normals(xyz, path, n_points, k, subsample), xyz, rgb)
-
-
-def _with_normals(xyz, path, n_points, k, subsample):
-    """Normals of every point of xyz on the GPU, then the subset: (4096, 6) rows."""
-    from meshanything_b200.normals import estimate_normals
-    normals = estimate_normals(xyz, k).cpu().numpy()
-    if subsample == 'fps':
-        keep = _farthest_points(xyz, path, n_points)
-    else:
-        keep = np.random.choice(xyz.shape[0], n_points, replace=False)
-    return np.concatenate([xyz[keep], normals[keep].astype(xyz.dtype)], axis=1)
+    assert xyz.shape[0] >= n_points, "input pc_normal should have at least 4096 points"
+    parts = [slice(None)] if objects is None else _split_objects(xyz, path, objects, n_points)
+    uid = _uid_of(path)
+    entries = []
+    for j, part in enumerate(parts):
+        obj = xyz[part]
+        obj_normals = estimate_normals(obj, k).cpu().numpy() if normals is None else normals[part]
+        keep = (_farthest_points(obj, path, n_points) if subsample == 'fps'
+                else np.random.choice(obj.shape[0], n_points, replace=False))
+        entry = {'pc_normal': np.concatenate([obj[keep], obj_normals[keep].astype(obj.dtype)], axis=1),
+                 'uid': uid if objects is None else f"{uid}_obj{j}"}
+        if rgb is not None:
+            entry['colors'] = np.concatenate([np.asarray(obj, dtype=np.float64), rgb[part]], axis=1)
+        entries.append(entry)
+    return entries
 
 
 def _vertex_colors(item, vertices, faces, output_frame, distance):
@@ -221,81 +167,49 @@ def _uid_of(path):
     return path.split('/')[-1].split('.')[0]
 
 
-_NO_MESH_OUTLIERS = ("--remove_outliers applies to point-cloud input (--input_type pc or pc_normal): the points of a "
-                     "mesh are sampled from its surface and have no outliers")
-_NO_MESH_FPS = ("--subsample fps applies to point-cloud input (--input_type pc or pc_normal): the points of a mesh are "
-                "already sampled uniformly by area")
-_NO_MESH_OBJECTS = ("--split_objects applies to point-cloud input (--input_type pc or pc_normal): splitting a mesh into "
-                    "its connected parts is not supported")
-_NO_MESH_SMOOTH = ("--smooth applies to point-cloud input (--input_type pc or pc_normal): the points of a mesh are "
-                   "sampled exactly from its surface and carry no scanner noise")
-_NO_MESH_COLORS = ("--transfer_colors applies to point-cloud input (--input_type pc or pc_normal): colours of a mesh's "
-                   "own vertices or textures are not read")
-_NO_MESH_PLANE = ("--remove_plane applies to point-cloud input (--input_type pc or pc_normal): the points of a mesh are "
-                  "sampled from its own surface, which has no scanned support under it")
 SUBSAMPLERS = ('random', 'fps')
 OUTPUT_FRAMES = ('model', 'input')
 
 
-def _check_subsample(input_type, subsample):
+def _subsampler(subsample):
     if subsample not in SUBSAMPLERS:
         raise ValueError(f"--subsample must be one of {', '.join(SUBSAMPLERS)}, got {subsample!r}")
-    if subsample == 'fps' and input_type not in ('pc', 'pc_normal'):
-        raise ValueError(_NO_MESH_FPS)
+    return subsample
+
+
+def _on(value):
+    """Whether a Dataset argument of STAGES runs its stage: off is None, False or 'random'."""
+    return value not in (None, False, 'random')
 
 
 class Dataset:
     """Same contract as the reference's Dataset (main.py:15-58): items are {'pc_normal': fp16 (4096, 6), 'uid': str},
-    coordinates centred on the bounding box and scaled to max |x| = 0.9995, unit normals asserted.  `outliers` (point
-    clouds only): None, or the keyword arguments of meshanything_b200.outliers.remove_outliers, to clean every cloud
-    before normals and subset.  `subsample` (point clouds only): 'random' (the reference's np.random.choice) or 'fps'
-    (farthest-point sampling on the GPU, DESIGN.md section 1.4).  `plane` (point clouds only): None, or the keyword
-    arguments of meshanything_b200.plane.remove_plane, to remove the support plane (a table, the floor) first.
-    `objects` (point clouds only): None, or {'distance': e}, to split every cloud after plane and outlier removal into
-    objects (DESIGN.md section 1.7), each its own item with uid `{uid}_obj{k}`.  `smooth` (point clouds only): None, or
-    {'k': k}, to smooth every cloud after plane and outlier removal (DESIGN.md section 1.8; for pc_normal only the xyz
-    columns move).  Items also carry 'frame', the
-    metrics.shape_frame of the rows before normalisation, which metrics.to_input_frame applies to put a mesh back in
-    the input's coordinates.  `colors` (point clouds only, `--transfer_colors`): read the files' colours, and give every
-    item a 'colors' entry, float64 [M, 6]: the full cleaned cloud it was drawn from (after plane and outlier removal,
-    smoothing and splitting; not the 4096-point subset), xyz in the input's units | rgb in [0, 1]."""
+    coordinates centred on the bounding box and scaled to max |x| = 0.9995, unit normals asserted; they also carry
+    'frame', the metrics.shape_frame of the rows before normalisation, which metrics.to_input_frame applies to put a
+    mesh back in the input's coordinates.  The other arguments are the optional stages of point-cloud input (STAGES,
+    refused for meshes; _cloud_items runs them): `outliers` None or the keyword arguments of
+    meshanything_b200.outliers.remove_outliers (DESIGN.md section 1.3), `subsample` 'random' (the reference's
+    np.random.choice) or 'fps' (section 1.4), `plane` None or those of meshanything_b200.plane.remove_plane (section
+    1.6), `objects` None or {'distance': e} (section 1.7), `smooth` None or {'k': k} (section 1.8), and `colors`
+    (section 1.9): give every item a 'colors' entry, float64 [M, 6], the full cleaned cloud it was drawn from (not the
+    4096-point subset), xyz in the input's units | rgb in [0, 1]."""
 
     def __init__(self, input_type, input_list, mc=False, outliers=None, subsample='random', plane=None, objects=None,
                  smooth=None, colors=False):
-        if outliers is not None and input_type not in ('pc', 'pc_normal'):
-            raise ValueError(_NO_MESH_OUTLIERS)
-        if plane is not None and input_type not in ('pc', 'pc_normal'):
-            raise ValueError(_NO_MESH_PLANE)
-        if objects is not None and input_type not in ('pc', 'pc_normal'):
-            raise ValueError(_NO_MESH_OBJECTS)
-        if smooth is not None and input_type not in ('pc', 'pc_normal'):
-            raise ValueError(_NO_MESH_SMOOTH)
-        if colors and input_type not in ('pc', 'pc_normal'):
-            raise ValueError(_NO_MESH_COLORS)
-        _check_subsample(input_type, subsample)
-        kw = dict(outliers=outliers, subsample=subsample, plane=plane, objects=objects)
-        if smooth is not None:
-            kw['smooth'] = smooth
-        if colors:
-            kw['colors'] = True
-        if input_type == 'pc_normal':
-            clouds = [_subsample_points(p, **kw) for p in input_list]
-        elif input_type == 'pc':
-            clouds = [_points_with_normals(p, **kw) for p in input_list]
-        elif input_type == 'mesh':
+        options = dict(outliers=outliers, subsample=_subsampler(subsample), plane=plane, objects=objects,
+                       smooth=smooth, colors=colors)
+        if input_type in ('pc', 'pc_normal'):
+            self.data = [entry for p in input_list for entry in _cloud_items(input_type, p, **options)]
+        else:
+            for keyword, stage in STAGES.items():
+                if _on(options[keyword]):
+                    raise ValueError(stage.refusal)
+            if input_type != 'mesh':
+                raise ValueError(f"unknown input_type {input_type!r}")
             if mc:
                 print("First Marching Cubes and then sample point cloud, need several minutes...")
             clouds, _ = process_mesh_to_pc([load_mesh(p) for p in input_list], marching_cubes=mc)
-        else:
-            raise ValueError(f"unknown input_type {input_type!r}")
-        if objects is None:
             self.data = [{'pc_normal': c, 'uid': _uid_of(p)} for c, p in zip(clouds, input_list)]
-        else:
-            self.data = [{'pc_normal': c, 'uid': f"{_uid_of(p)}_obj{k}"}
-                         for cs, p in zip(clouds, input_list) for k, c in enumerate(cs)]
-        if colors:
-            for entry in self.data:
-                entry['pc_normal'], entry['colors'] = entry['pc_normal']
         print(f"dataset total data samples: {len(self.data)}")
 
     def __len__(self):
@@ -320,7 +234,7 @@ _FLAGS = [  # (flag, default, type) -- the reference's command line (main.py:60-
 ]
 
 
-def get_args():
+def _parser():
     parser = argparse.ArgumentParser("MeshAnything", add_help=False)
     for flag, default, typ in _FLAGS:
         parser.add_argument(flag, default=default, type=typ)
@@ -375,41 +289,92 @@ def get_args():
     parser.add_argument('--color_distance', default=0.05, type=float,
                         help="points farther than this share of the cloud's longest side from the mesh give no colour, "
                              "in (0, 1] (default 0.05)")
-    return parser.parse_args()
+    return parser
 
 
-def outlier_options(args):
-    """The `outliers` argument of Dataset from the command line: None without --remove_outliers."""
-    if not args.remove_outliers:
-        return None
-    return {'k': args.outlier_neighbors, 'std_ratio': args.outlier_std_ratio,
-            'min_component': args.outlier_min_component}
+def get_args():
+    return _parser().parse_args()
 
 
-def plane_options(args):
-    """The `plane` argument of Dataset from the command line: None without --remove_plane."""
-    if not getattr(args, 'remove_plane', False):
-        return None
-    return {'distance': getattr(args, 'plane_distance', 0.01), 'iterations': getattr(args, 'plane_iterations', 1000)}
+_DEFAULTS = vars(_parser().parse_args([]))
 
 
-def object_options(args):
-    """The `objects` argument of Dataset from the command line: None without --split_objects."""
-    if not getattr(args, 'split_objects', False):
-        return None
-    return {'distance': getattr(args, 'object_distance', 0.02)}
+def _arg(args, name):
+    """args.<name>, or the command line's default for a namespace built without that flag."""
+    return getattr(args, name, _DEFAULTS[name])
 
 
-def smooth_options(args):
-    """The `smooth` argument of Dataset from the command line: None without --smooth."""
-    if not getattr(args, 'smooth', False):
-        return None
-    return {'k': getattr(args, 'smooth_neighbors', 24)}
+def _options(flag, **names):
+    """args -> {key: args.<name>} of a stage turned on by --<flag>, or None when it is off."""
+    return lambda args: {key: _arg(args, name) for key, name in names.items()} if _arg(args, flag) else None
 
 
-def color_options(args):
-    """The `colors` argument of Dataset from the command line."""
-    return bool(getattr(args, 'transfer_colors', False))
+def _check_share(args, name, square=False):
+    """--<name> is a share of the bounding box's longest side: in (0, 1], and above 0 in fp32 (with `square` its
+    square, which is what the kernel compares)."""
+    d = _arg(args, name)
+    if not (np.isfinite(d) and 0 < d <= 1 and (np.float32(d) * np.float32(d) if square else np.float32(d)) > 0):
+        raise ValueError(f"--{name} must be in (0, 1] (a share of the bounding box's longest side"
+                         f"{', with a square above 0 in fp32' if square else ''}), got {d}")
+
+
+def _check_outliers(args):
+    k, std_ratio, min_component = (_arg(args, 'outlier_' + s) for s in ('neighbors', 'std_ratio', 'min_component'))
+    if not 1 <= k <= 64:
+        raise ValueError(f"--outlier_neighbors must be in 1..64, got {k}")
+    if not (np.isfinite(std_ratio) and np.isfinite(min_component) and min_component >= 0):
+        raise ValueError("--outlier_std_ratio must be finite and --outlier_min_component finite and >= 0")
+
+
+def _check_plane(args):
+    _check_share(args, 'plane_distance')
+    iterations = _arg(args, 'plane_iterations')
+    if not 1 <= iterations <= capi.PLANE_MAX_H:
+        raise ValueError(f"--plane_iterations must be in 1..{capi.PLANE_MAX_H}, got {iterations}")
+
+
+def _check_smooth(args):
+    k = _arg(args, 'smooth_neighbors')
+    if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not capi.SMOOTH_MIN_K <= k <= 64:
+        raise ValueError(f"--smooth_neighbors must be in {capi.SMOOTH_MIN_K}..64, got {k}")
+
+
+class _Stage(NamedTuple):
+    flag: str            # what turns the stage on, as the messages name it
+    options: Callable    # args -> its Dataset argument; _on tells whether that runs the stage
+    check: Callable      # args -> ValueError for options out of range (called when the stage runs)
+    mesh: str            # why mesh input is refused
+
+    @property
+    def refusal(self):
+        return f"{self.flag} applies to point-cloud input (--input_type pc or pc_normal): {self.mesh}"
+
+
+# The optional stages of point-cloud input by their Dataset argument, in the order check_args checks them.
+STAGES = {
+    'outliers': _Stage('--remove_outliers', _options('remove_outliers', k='outlier_neighbors',
+                                                      std_ratio='outlier_std_ratio',
+                                                      min_component='outlier_min_component'), _check_outliers,
+                       "the points of a mesh are sampled from its surface and have no outliers"),
+    'subsample': _Stage('--subsample fps', lambda args: _subsampler(_arg(args, 'subsample')), lambda args: None,
+                        "the points of a mesh are already sampled uniformly by area"),
+    'plane': _Stage('--remove_plane', _options('remove_plane', distance='plane_distance',
+                                                iterations='plane_iterations'), _check_plane,
+                    "the points of a mesh are sampled from its own surface, which has no scanned support under it"),
+    'objects': _Stage('--split_objects', _options('split_objects', distance='object_distance'),
+                      lambda args: _check_share(args, 'object_distance', square=True),
+                      "splitting a mesh into its connected parts is not supported"),
+    'smooth': _Stage('--smooth', _options('smooth', k='smooth_neighbors'), _check_smooth,
+                     "the points of a mesh are sampled exactly from its surface and carry no scanner noise"),
+    'colors': _Stage('--transfer_colors', lambda args: bool(_arg(args, 'transfer_colors')),
+                     lambda args: _check_share(args, 'color_distance'),
+                     "colours of a mesh's own vertices or textures are not read"),
+}
+outlier_options = STAGES['outliers'].options
+plane_options = STAGES['plane'].options
+object_options = STAGES['objects'].options
+smooth_options = STAGES['smooth'].options
+color_options = STAGES['colors'].options
 
 
 def check_args(args):
@@ -420,46 +385,12 @@ def check_args(args):
     if args.num_samples > 1 and args.continuous_batching:
         raise ValueError("--num_samples > 1 does not run with --continuous_batching: best-of-N scores the candidates "
                          "of a padded batch together")
-    if args.remove_outliers:
-        if args.input_type == 'mesh':
-            raise ValueError(_NO_MESH_OUTLIERS)
-        if not 1 <= args.outlier_neighbors <= 64:
-            raise ValueError(f"--outlier_neighbors must be in 1..64, got {args.outlier_neighbors}")
-        if not (np.isfinite(args.outlier_std_ratio) and np.isfinite(args.outlier_min_component)
-                and args.outlier_min_component >= 0):
-            raise ValueError("--outlier_std_ratio must be finite and --outlier_min_component finite and >= 0")
-    _check_subsample(args.input_type, getattr(args, 'subsample', 'random'))   # namespaces built without the flag
-    if getattr(args, 'remove_plane', False):
-        if args.input_type == 'mesh':
-            raise ValueError(_NO_MESH_PLANE)
-        distance = getattr(args, 'plane_distance', 0.01)
-        iterations = getattr(args, 'plane_iterations', 1000)
-        if not (np.isfinite(distance) and 0 < distance <= 1 and np.float32(distance) > 0):
-            raise ValueError(f"--plane_distance must be in (0, 1] (a share of the bounding box's longest side), got "
-                             f"{distance}")
-        if not 1 <= iterations <= 65536:
-            raise ValueError(f"--plane_iterations must be in 1..65536, got {iterations}")
-    if getattr(args, 'split_objects', False):
-        if args.input_type == 'mesh':
-            raise ValueError(_NO_MESH_OBJECTS)
-        distance = getattr(args, 'object_distance', 0.02)
-        if not (np.isfinite(distance) and 0 < distance <= 1 and np.float32(distance) * np.float32(distance) > 0):
-            raise ValueError(f"--object_distance must be in (0, 1] (a share of the bounding box's longest side, with a "
-                             f"square above 0 in fp32), got {distance}")
-    if getattr(args, 'smooth', False):
-        if args.input_type == 'mesh':
-            raise ValueError(_NO_MESH_SMOOTH)
-        k = getattr(args, 'smooth_neighbors', 24)
-        if isinstance(k, bool) or not isinstance(k, (int, np.integer)) or not 5 <= k <= 64:
-            raise ValueError(f"--smooth_neighbors must be in 5..64, got {k}")
-    if getattr(args, 'transfer_colors', False):
-        if args.input_type == 'mesh':
-            raise ValueError(_NO_MESH_COLORS)
-        distance = getattr(args, 'color_distance', 0.05)
-        if not (np.isfinite(distance) and 0 < distance <= 1 and np.float32(distance) > 0):
-            raise ValueError(f"--color_distance must be in (0, 1] (a share of the bounding box's longest side), got "
-                             f"{distance}")
-    if getattr(args, 'output_frame', 'model') not in OUTPUT_FRAMES:
+    for stage in STAGES.values():
+        if _on(stage.options(args)):
+            if args.input_type == 'mesh':
+                raise ValueError(stage.refusal)
+            stage.check(args)
+    if _arg(args, 'output_frame') not in OUTPUT_FRAMES:
         raise ValueError(f"--output_frame must be one of {', '.join(OUTPUT_FRAMES)}, got {args.output_frame!r}")
 
 
@@ -595,9 +526,7 @@ if __name__ == "__main__":
         raise ValueError("input_dir or input_path must be provided.")
     np.random.seed(args.seed)
     torch.manual_seed(args.seed)
-    dataset = Dataset(args.input_type, input_list, args.mc, outliers=outlier_options(args), subsample=args.subsample,
-                      plane=plane_options(args), objects=object_options(args), smooth=smooth_options(args),
-                      colors=color_options(args))
+    dataset = Dataset(args.input_type, input_list, args.mc, **{k: stage.options(args) for k, stage in STAGES.items()})
 
     bs = args.batchsize_per_gpu
     batches = [list(range(i, min(i + bs, len(dataset)))) for i in range(0, len(dataset), bs)]

@@ -218,6 +218,26 @@ def load_points(path, colors=False):
     raise ValueError(f"{path}: --input_type pc reads .npy (N, 3) and vertex-only .ply files")
 
 
+def load_cloud(path, input_type, colors=False):
+    """A point-cloud file as (xyz [N, 3], normals or None, rgb float64 [N, 3] in [0, 1] or None), rows aligned.
+
+    `pc`: a bare cloud (load_points), integer xyz as float64; no normals.  `pc_normal`: an .npy of (xyz, normal) rows,
+    both in the file's dtype.  With `colors` (`--transfer_colors`) also the colours: for pc as load_points reads them,
+    for pc_normal from an (N, 9) .npy, xyz | normal | rgb."""
+    if input_type == 'pc':
+        xyz, rgb = load_points(path, colors=True) if colors else (load_points(path), None)
+        if not np.issubdtype(xyz.dtype, np.floating):
+            xyz = xyz.astype(np.float64)
+        return xyz, None, rgb
+    cloud, rgb = np.load(path), None
+    if colors:
+        if cloud.ndim != 2 or cloud.shape[1] != 9:
+            raise ValueError(f"{path}: --transfer_colors reads a coloured pc_normal cloud as an array of shape (N, 9), "
+                             f"xyz | normal | rgb, got {cloud.shape}")
+        cloud, rgb = cloud[:, :6], check_rgb(path, cloud[:, 6:])
+    return cloud[:, :3], cloud[:, 3:], rgb
+
+
 def load_mesh(path):
     if trimesh is not None:
         return trimesh.load(path)

@@ -238,12 +238,12 @@ def test_npy_colour_layouts(tmp_path, monkeypatch):
     import main as cli
     np.save(tmp_path / "pcn.npy", np.concatenate([xyz, nrm, rgb], 1))
     np.random.seed(0)
-    sub, cloud = cli._subsample_points(str(tmp_path / "pcn.npy"), colors=True)
-    assert sub.shape == (4096, 6) and np.array_equal(cloud, np.concatenate([xyz, rgb], 1))
+    entry = cli.Dataset("pc_normal", [str(tmp_path / "pcn.npy")], colors=True).data[0]
+    assert entry["pc_normal"].shape == (4096, 6) and np.array_equal(entry["colors"], np.concatenate([xyz, rgb], 1))
 
 
 def test_refusals(tmp_path, monkeypatch):
-    from mesh_to_pc import load_points
+    from mesh_to_pc import load_cloud, load_points
     monkeypatch.syspath_prepend(ROOT)
     import main as cli
     rng = np.random.default_rng(8)
@@ -276,7 +276,7 @@ def test_refusals(tmp_path, monkeypatch):
     for shape in ((5000, 6), (5000, 3)):
         np.save(tmp_path / "n9.npy", np.zeros(shape))
         with pytest.raises(ValueError, match=r"\(N, 9\), xyz \| normal \| rgb"):
-            cli._subsample_points(str(tmp_path / "n9.npy"), colors=True)
+            load_cloud(str(tmp_path / "n9.npy"), "pc_normal", colors=True)
     # without the flag the loaders' messages are unchanged
     np.save(tmp_path / "six.npy", np.zeros((20, 6)))
     with pytest.raises(ValueError, match="looks like points with normals"):
